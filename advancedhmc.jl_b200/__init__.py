@@ -1,4 +1,4 @@
-"""advancedhmc.jl_b200 -- B200-native (sm_100a) many-chain leapfrog / HMC / NUTS engine behind
+"""advancedhmc.jl_b200 -- H100-native (sm_90a) many-chain leapfrog / HMC / NUTS engine behind
 AdvancedHMC.jl's `AbstractIntegrator` / `Hamiltonian` / `AbstractMetric` plugin surface.
 
 The directory name is not a legal Python identifier; import it as `ahmc_b200` (root-level shim).

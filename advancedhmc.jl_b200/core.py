@@ -47,8 +47,8 @@ class Context:
         rc = self.lib.ahmc_create(C.byref(h), device, C.c_void_p(stream) if stream else None)
         if rc != L.OK:
             raise RuntimeError(
-                f"ahmc_create(device={device}) failed with code {rc}: libahmc_b200 needs a CUDA device "
-                "(there is no CPU fallback; the CPU restatement under oracle/ is test infrastructure only)")
+                f"ahmc_create(device={device}) failed with code {rc}: libahmc_b200 needs a CUDA device of compute "
+                "capability 9.0, the sm_90a code it is built for (there is no CPU fallback; the CPU restatement under oracle/ is test infrastructure only)")
         self.h = h
 
     def check(self, rc: int):
@@ -1074,7 +1074,7 @@ def adapt_cov(theta, mean):
 
 # ------------------------------------------------------------------------------------------------
 # deployment helper: host-buffer calls move every byte over PCIe, so the page-locked buffers should live on the NUMA
-# node the GPU hangs off (on a two-socket B200 box a remote node costs up to ~1.5x per call, profiles/README.md)
+# node the GPU hangs off (on a two-socket host a buffer on the remote node slows every call)
 # ------------------------------------------------------------------------------------------------
 def bind_to_gpu_numa(device: int = 0):
     """Pin the calling thread to the CPUs NVML reports as local to `device` (nvmlDeviceSetCpuAffinity) so that memory

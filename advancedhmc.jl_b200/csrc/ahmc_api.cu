@@ -10,11 +10,10 @@
 #include <string>
 #include <vector>
 
-// defaults of the host-buffer lane (see leapfrog_host_pipelined), chosen by measurement on B200 (profiles/README.md,
-// "host-buffer lane"): page-locked buffers are read and written by the kernel directly in ONE launch whose residency
-// is capped at one CTA per SM, so the grid runs in staggered waves and uploads overlap downloads (0.36 ms against
-// 0.48 ms uncapped and 0.45-0.50 ms for the best copy-engine pipeline at 4096 x 128); pageable buffers go through
-// the copy engines in two chunks.
+// defaults of the host-buffer lane (see leapfrog_host_pipelined): page-locked buffers are read and written by the kernel
+// directly in ONE launch whose residency is capped at one CTA per SM, so the grid runs in staggered waves and uploads
+// overlap downloads; pageable buffers go through the copy engines in two chunks.  The first calls of a shape measure the
+// candidate transports and keep the fastest.
 #define AHMC_PIPE_DIRECT_CHUNKS 1
 #define AHMC_PIPE_CE_CHUNKS 2
 #define AHMC_PIPE_DIRECT_OCC 1  // resident CTAs per SM of a direct-access launch (0 = no cap)
@@ -25,6 +24,7 @@ using namespace ahmc;
 
 struct ahmc_ctx {
     int device = 0;
+    int sm_count = 0;  // streaming multiprocessors of the device (grid size of the one-wave reductions)
     cudaStream_t stream = nullptr;
     bool own_stream = false;
     std::string err;
@@ -420,7 +420,7 @@ int try_dense_trajectory(ahmc_ctx* ctx, const ahmc_model* model, LeapfrogArgs& a
 // =================================================================================================
 extern "C" {
 
-const char* ahmc_version(void) { return "ahmc_b200 0.1.0 (sm_100a)"; }
+const char* ahmc_version(void) { return "ahmc_b200 0.1.0 (sm_90a)"; }
 
 int ahmc_create(ahmc_ctx** out, int32_t device, void* cuda_stream) {
     if (!out) return AHMC_ERR_INVALID;
@@ -436,6 +436,17 @@ int ahmc_create(ahmc_ctx** out, int32_t device, void* cuda_stream) {
         delete ctx;
         return AHMC_ERR_CUDA;
     }
+    int cc_major = 0, cc_minor = 0;
+    cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, device);
+    cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, device);
+    if (cc_major != 9 || cc_minor != 0) {
+        // the library holds sm_90a code only, which runs on compute capability 9.0 (H100 / H200) and nothing else
+        fprintf(stderr, "ahmc_create: device %d has compute capability %d.%d; libahmc_b200 is built for sm_90a (9.0)\n", device,
+                cc_major, cc_minor);
+        delete ctx;
+        return AHMC_ERR_UNSUPPORTED;
+    }
+    cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device);
     DeviceGuard g(device);
     if (cuda_stream) {
         ctx->stream = (cudaStream_t)cuda_stream;
@@ -765,11 +776,10 @@ static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const
     bool down_direct = out_pinned;
     int occ_cap = AHMC_PIPE_DIRECT_OCC;
     int nchunk = 0;
-    // ---- transport choice.  Page-locked buffers can be moved in several ways whose ranking depends on the HOST (the
-    // zero-copy lane measured 0.36 ms on one box and 3.8 ms on another: SM-issued reads of system memory are at the mercy
-    // of the platform's read-completion latency, copy engines are not), so the first calls of a given shape try each
-    // candidate in turn -- results are bit-identical in every mode, nothing extra is executed -- and the fastest is kept
-    // for the life of the context.  Candidates: {direct loads + direct stores, 1 CTA/SM}, {copy engines, 2 / 4 chunks},
+    // ---- transport choice.  Page-locked buffers can be moved in several ways whose ranking depends on the HOST
+    // (SM-issued reads of system memory are at the mercy of the platform's read-completion latency, copy engines are
+    // not), so the first calls of a given shape try each candidate in turn -- results are bit-identical in every mode,
+    // nothing extra is executed -- and the fastest is kept for the life of the context.  Candidates: {direct loads + direct stores, 1 CTA/SM}, {copy engines, 2 / 4 chunks},
     // {copy-engine upload, direct stores, 4 chunks}.  The AHMC_PIPE_* variables pin the choice (A/B runs).
     struct Cand { int up; bool down_direct; int chunks; int occ; };
     static const Cand kCands[] = {{UP_DIRECT, true, 1, 1}, {UP_CE1, false, 2, 0}, {UP_CE1, false, 4, 0}, {UP_CE1, true, 4, 1}};
@@ -1669,7 +1679,7 @@ int ahmc_adapt_summary_f64(ahmc_ctx* ctx, int32_t D, int64_t N, const double* th
     if (!ctx || !theta || !out) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/theta/out");
     if (D < 1 || N < 1 || ld < D) return fail(ctx, AHMC_ERR_INVALID, "need D >= 1, N >= 1, ld >= D");
     DeviceGuard g(ctx->device);
-    const int blocks = (int)(N < 148 ? N : 148);
+    const int blocks = (int)(N < ctx->sm_count ? N : ctx->sm_count);
     const size_t need = ((size_t)blocks * (D + 1) + 2) * sizeof(double);
     if (need > ctx->adapt_scratch_bytes) {
         CU(cudaStreamSynchronize(ctx->stream));
@@ -1907,7 +1917,7 @@ int ahmc_adapt_exchange_f64(ahmc_ctx* ctx, ahmc_comm* comm, ahmc_pooled* a, int3
         a->gathered_ranks = R;
     }
     // K5: this rank's record (same workspace discipline as ahmc_adapt_summary_f64)
-    const int blocks = (int)(N < 148 ? N : 148);
+    const int blocks = (int)(N < ctx->sm_count ? N : ctx->sm_count);
     const size_t need = ((size_t)blocks * (D + 1) + 2) * sizeof(double);
     if (need > ctx->adapt_scratch_bytes) {
         CU(cudaStreamSynchronize(ctx->stream));

@@ -22,14 +22,14 @@ namespace ahmc {
 
 constexpr int kDenseThreads = 256;  // 8 warps
 constexpr int kKC = 16;             // columns of A per pipeline stage
-// A pipeline (measured on B200 in round 2, profiles/r02/k4_ab.md: 15.0 -> 20.2 TFLOP/s at 4096 x 128, 16.0 -> 24.7 at 16384):
+// A pipeline:
 //   * the padded matrix is stored with the shared-memory stage's leading dimension (Dp + 4, ahmc_kernels.cuh dense_lda), so a
 //     16-column chunk is ONE contiguous bulk copy instead of sixteen;
 //   * consumers release a stage through an "empty" mbarrier (one arrival per warp) and only the producer thread waits on it,
 //     instead of a CTA-wide __syncthreads per chunk;
 //   * three stages.  Shared memory: 68 KB per CTA at Dp = 128 (two CTAs per SM still fit), 232,272 of the 232,448 bytes a CTA
 //     may have at Dp = 512.
-constexpr int kStages = 3;  // 4 and 5 stages measured no faster (profiles/r02/k4_stages_ab.log): the wait is L2 latency per chunk, not depth
+constexpr int kStages = 3;  // the wait is L2 latency per chunk, not pipeline depth
 constexpr int kBars = 2 * kStages;  // full[kStages] + empty[kStages]
 #ifdef AHMC_SIMT_EMULATION
 extern unsigned char* emu_dynamic_smem;  // the block's dynamic shared memory (blocks run one at a time)
@@ -437,9 +437,8 @@ cudaError_t launch_dense_traj(const DenseTrajHost& h, cudaStream_t st, int* n_la
     switch (RB) {
         case 1: return launch_dense_t<1, 4>(a, st);
         case 2: {
-            // D <= 128: tiles of 16 chains, two CTAs per SM -- the barrier / copy waits of one hide behind the other
-            // (measured on B200, 4096 / 16384 chains x D=128, L=32: 0.286 / 1.07 ms against 0.294 / 1.91 ms for one
-            // 32-chain CTA per SM).  AHMC_DENSE_TILE=32x1 selects the single-CTA form for A/B runs.
+            // D <= 128: tiles of 16 chains, two CTAs per SM -- the barrier / copy waits of one hide behind the other.
+            // AHMC_DENSE_TILE=32x1 selects the single-CTA form (one 32-chain CTA per SM) for A/B runs.
             const char* ev = getenv("AHMC_DENSE_TILE");
             if (ev && !strcmp(ev, "32x1")) return launch_dense_t<2, 4>(a, st);
             return launch_dense_t<2, 2, 2>(a, st);

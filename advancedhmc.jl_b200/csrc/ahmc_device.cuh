@@ -1,4 +1,4 @@
-// ahmc_device.cuh -- device-side building blocks shared by every kernel of libahmc_b200 (sm_100a).
+// ahmc_device.cuh -- device-side building blocks shared by every kernel of libahmc_b200 (sm_90a).
 //
 // Work decomposition ("group-distributed vectors"): one chain is owned by a GROUP of G consecutive
 // lanes of a warp (G in {4,8,16,32}); lane l of the group holds E coordinates d = l + G*e, e < E, so a
@@ -140,10 +140,10 @@ __device__ __forceinline__ void vstore(double* base, const double (&x)[E], int l
 
 // ------------------------------------------------------------------------------------------------
 // lane-contiguous vector I/O (K1 fast path, G = 32): lane l owns V = min(E, 4) CONSECUTIVE doubles of every
-// 32*V-wide block, element e  <->  d = 32*V*(e / V) + V*l + (e % V).  One 128-bit (V = 2) or 256-bit (V = 4,
-// LDG.E.256 / STG.E.256 on sm_100) access per lane per block instead of V scalar ones; a warp instruction still
-// covers one contiguous run of 32*V doubles.  Used for FULL tiles only (D == 32*E, 8*V-byte aligned rows; the host
-// checks): no bounds predicate, no zero fill.
+// 32*V-wide block, element e  <->  d = 32*V*(e / V) + V*l + (e % V).  A lane moves its V doubles with 128-bit
+// accesses instead of V scalar ones (sm_90 has no wider per-thread load or store: V = 4 is two of them, at d0 and
+// d0 + 2).  Used for FULL tiles only (D == 32*E, 8*V-byte aligned rows; the host checks): no bounds predicate, no
+// zero fill.
 // ------------------------------------------------------------------------------------------------
 template <int E>
 struct Contig {
@@ -157,13 +157,9 @@ __device__ __forceinline__ void cload(double (&x)[E], const double* base, int l,
     for (int b = 0; b < E / V; ++b) {
         const int d0 = 32 * V * b + V * l;
         if constexpr (V == 4) {
-#if defined(AHMC_SIMT_EMULATION)
-            for (int j = 0; j < 4; ++j) x[4 * b + j] = base[d0 + j];
-#else
-            asm volatile("ld.global.v4.f64 {%0,%1,%2,%3}, [%4];"
-                         : "=d"(x[4 * b]), "=d"(x[4 * b + 1]), "=d"(x[4 * b + 2]), "=d"(x[4 * b + 3])
-                         : "l"(base + d0));
-#endif
+            const double2 v0 = *reinterpret_cast<const double2*>(base + d0);
+            const double2 v1 = *reinterpret_cast<const double2*>(base + d0 + 2);
+            x[4 * b] = v0.x; x[4 * b + 1] = v0.y; x[4 * b + 2] = v1.x; x[4 * b + 3] = v1.y;
         } else if constexpr (V == 2) {
             double2 v = *reinterpret_cast<const double2*>(base + d0);
             x[2 * b] = v.x; x[2 * b + 1] = v.y;
@@ -179,12 +175,8 @@ __device__ __forceinline__ void cstore(double* base, const double (&x)[E], int l
     for (int b = 0; b < E / V; ++b) {
         const int d0 = 32 * V * b + V * l;
         if constexpr (V == 4) {
-#if defined(AHMC_SIMT_EMULATION)
-            for (int j = 0; j < 4; ++j) base[d0 + j] = x[4 * b + j];
-#else
-            asm volatile("st.global.v4.f64 [%0], {%1,%2,%3,%4};" ::"l"(base + d0), "d"(x[4 * b]), "d"(x[4 * b + 1]),
-                         "d"(x[4 * b + 2]), "d"(x[4 * b + 3]) : "memory");
-#endif
+            *reinterpret_cast<double2*>(base + d0) = make_double2(x[4 * b], x[4 * b + 1]);
+            *reinterpret_cast<double2*>(base + d0 + 2) = make_double2(x[4 * b + 2], x[4 * b + 3]);
         } else if constexpr (V == 2) {
             *reinterpret_cast<double2*>(base + d0) = make_double2(x[2 * b], x[2 * b + 1]);
         } else {
@@ -246,7 +238,7 @@ __device__ __forceinline__ void matvec(const double* __restrict__ A, int D, cons
 // Under the CPU SIMT emulation the harness provides them with the same contracts (tests/simt_emu/simt_emu.cpp): an
 // mbarrier is (completed phases, pending arrivals, pending transaction bytes), `mbar_wait(parity)` returns once the phase
 // of that parity has completed, `bulk_g2s` copies synchronously and completes its bytes on the barrier, `dmma` is
-// mma.sync.aligned.m8n8k4.row.col.f64 (tcgen05 has no f64 kind): lane l holds A[l/4][l%4], B[l%4][l/4], C[l/4][2(l%4)+{0,1}].
+// mma.sync.aligned.m8n8k4.row.col.f64 (wgmma has no f64 kind): lane l holds A[l/4][l%4], B[l%4][l/4], C[l/4][2(l%4)+{0,1}].
 // ------------------------------------------------------------------------------------------------
 #ifdef AHMC_SIMT_EMULATION
 void mbar_init(uint64_t* bar, int count);
@@ -311,8 +303,7 @@ __device__ __forceinline__ void dmma(double& d0, double& d1, double a, double b)
 // 4 columns fall into distinct banks) | 16 doubles of slack | 2 coop_stages(D) mbarriers.  Idle warps still take part.
 // ------------------------------------------------------------------------------------------------
 // matrix columns per stage = per bulk copy and per pair of barrier operations, by the kernel's layout (E coordinates per
-// lane, D <= 32 E).  Measured on the C5 shape (D = 256, steps x dims/s): 8 columns x 6 stages 5.8e9, 16 x 4 8.2e9,
-// 24 x 3 8.6e9, 32 x 2 6.9e9; beyond D = 256 the stages must shrink to fit 227 KB.
+// lane, D <= 32 E).  Beyond D = 256 the stages must shrink to fit the 227 KB of shared memory a block may have.
 template <int E>
 __host__ __device__ constexpr int coop_kc() { return E <= 8 ? 24 : 16; }
 // stages of the L2 -> shared-memory pipeline (stages - 1 chunks in flight): the kernels that use it run one block per SM,
@@ -328,7 +319,7 @@ __host__ __device__ constexpr int coop_smem_doubles(int D, int KC) { return 2 * 
 // `full`.  Called by ALL lanes of warp 0, converged.  bulk: 16-byte aligned source columns and an even number of rows.
 // `padded` (nullable): the same columns in a copy of the matrix whose leading dimension already is coop_lds(D) -- the chunk
 // is then ONE contiguous bulk copy instead of one per column (a bulk copy costs the copy engine of the SM a fixed time
-// that 2 KB does not amortise: 3.8e9 -> 5.0e9 steps x dims/s on the C5 shape, even with unpadded, bank-conflicting stages).
+// that 2 KB does not amortise).
 __device__ __forceinline__ void coop_issue(double* stage, const double* __restrict__ src, const double* __restrict__ padded, int ncols,
                                            int rows, int D, bool bulk, uint64_t* full) {
     const int lane = threadIdx.x & 31;

@@ -89,10 +89,12 @@ struct StepIO {
     }
 };
 
-// Occupancy: the headline batch (4096 chains x D=128 -> 4096 warps) fits the chip in ONE wave only if 7 blocks of
-// 4 warps are resident per SM (148 x 7 x 4 = 4144 warp slots), i.e. <= 72 registers per thread.  The fast path needs
-// ~50; the cap makes the (rarely taken) exact fallback of the separable kernels spill a little, which is the right
-// trade.  Wider layouts (E >= 8) and non-separable models keep the default budget.
+// Occupancy: 7 blocks of 4 warps per SM, i.e. <= 72 registers per thread.  On an H100 (132 SMs x 7 x 4 = 3696 warp
+// slots) the headline batch (4096 chains x D=128 -> 4096 warps) runs as one full wave plus a 10 % tail.  Capping at 8
+// blocks (64 registers) would make it one wave but spills inside the fast path, and measured slower (H100 SXM, 400 W
+// power limit, L2 flushed: 14.5 against 14.4 us per launch at 4096 chains, 40.4 against 37.5 us at 16384).  The cap
+// makes the (rarely taken) exact fallback of the separable kernels spill a little, which is the right trade.  Wider
+// layouts (E >= 8) and non-separable models keep the default budget.
 template <int MODEL, int METRIC, int E>
 constexpr int min_blocks_per_sm() {
     return (FastCapable<MODEL, METRIC>::value && E <= 4) ? 7 : 1;
@@ -101,7 +103,7 @@ constexpr int min_blocks_per_sm() {
 // chains; capped it spills ~50 bytes outside the step loop and runs in one.  Its transition kernel would spill inside
 // the loop, so that one keeps the default.
 // The transition kernel of a general target: 128 registers (4 blocks per SM) are enough for E <= 4 without spills; left
-// alone it takes ~140 and loses a block per SM (measured on the funnel: 64 us per transition vs 53).
+// alone it takes ~140 and loses a block per SM.
 template <int MODEL, int METRIC, int E>
 constexpr int min_blocks_hmc() {
     return (FastCapable<MODEL, METRIC>::value && E <= 4) ? 7 : ((METRIC != AHMC_METRIC_DENSE && MODEL != AHMC_MODEL_DENSE_GAUSS && E <= 4) ? 4 : 1);

@@ -50,9 +50,8 @@ __device__ __forceinline__ double maxabs(double a, double b) { return fabs(a) > 
 
 constexpr int kLevelScalars = 7;  // lw (m), sum_alpha, n_alpha, dH_max, cand lp, cand lk, ww (w)
 
-// Instruction-count cuts taken from the K3 line profile (profiles/r01/k3_source_line_profile.txt: of 882 warp-instructions
-// per leaf, random draws 24 %, logaddexp 16 %, the leaf's exp 6 %), measured on B200 in round 2 (profiles/r02/k3_ab.md:
-// +44 % / +33 % on the C3 shape at eps = 0.1 / 0.4) and tape-identical to the recursive oracle:
+// Instruction-count cuts of the tree walk (random draws, logaddexp and the leaf's exp dominated it), tape-identical to the
+// recursive oracle:
 //   * variates are prefetched lane-parallel: lane l of the chain's group generates uniform #(base + l) of the Philox
 //     stream (one block per LANE instead of one per DRAW), a draw is then a group broadcast of one register; direction
 //     bits come from a cached block (128 doublings each);

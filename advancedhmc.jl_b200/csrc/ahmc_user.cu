@@ -167,7 +167,7 @@ static bool compile(UserModule* m, int which, int metric, int G, int E, UserModu
         return false;
     }
     g_rtc.AddNameExpression(prog, expr);
-    const char* opts[] = {"--gpu-architecture=sm_100a", "--std=c++17", "-default-device", "--fmad=true", "-lineinfo"};
+    const char* opts[] = {"--gpu-architecture=sm_90a", "--std=c++17", "-default-device", "--fmad=true", "-lineinfo"};
     rc = g_rtc.CompileProgram(prog, 5, opts);
     if (rc) {
         size_t n = 0;

@@ -1,13 +1,16 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 leapfrog engine (contract: see DESIGN.md "Measurement").
+"""bench.py -- headline benchmark of the H100 leapfrog engine (contract: see DESIGN.md "Measurement").
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" = one pass of the hot path over one batch: the fused L=32-step leapfrog trajectory
 (`step(Leapfrog(0.1), h, z, 32)`, src/integrator.jl:216-265) of 4096 chains x D=128 on a diagonal Gaussian
 target with a Diag-Euclidean metric -- the configuration BASELINE.json's metric is quoted on.
 Metric: leapfrog-steps*dims/s.  Weak scaling: every rank runs the same 4096-chain batch (chains shard
 with no data-path collective, SURVEY 8e), value = all ranks' units / max-over-ranks device time.
+--dump-outputs DIR writes what the last timed step returned (theta, r, lp value and gradient, lk value of the
+4096 x 128 phase point, float64, 12.6 MB) as DIR/<name>.npy; the inputs are seeded, so two builds can be
+compared output for output.
 """
 from __future__ import annotations
 
@@ -52,16 +55,7 @@ def peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def measured_traffic():
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02", "k1_headline_dram.json")) as f:
-            d = json.load(f)
-        return int(d["dram_bytes_read"] + d["dram_bytes_write"])
-    except Exception:
-        return None
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class Extra:
@@ -82,7 +76,7 @@ class Extra:
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (read-only queries)."""
 
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown," \
         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -245,7 +239,7 @@ def run_ours(args):
 
     with torch.cuda.stream(stream):
         z0 = A.phasepoint(h, torch.as_tensor(th, device=dev), torch.as_tensor(r, device=dev))
-        flush = torch.zeros(512 * 1024 * 1024 // 8, dtype=torch.float64, device=dev)  # 512 MiB > 126 MB L2
+        flush = torch.zeros(512 * 1024 * 1024 // 8, dtype=torch.float64, device=dev)  # 512 MiB >> the H100's 50 MB L2
 
         def flush_l2():
             # READ 512 MiB: fills L2 with clean lines of another buffer (a write-flush would leave it full of
@@ -274,6 +268,8 @@ def run_ours(args):
             ev[i][1].record(stream)
         torch.cuda.synchronize()
         launches = ctx.launches - l0
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, one_step.out)
         # keep the sampler alive for a moment of sustained load so clocks are seen under load
         t_end = time.time() + 0.4
         while time.time() < t_end:
@@ -526,7 +522,7 @@ def run_ours(args):
                 tf, msb = ctypes.c_double(), ctypes.c_double()
                 rcmb = mb.ahmc_mb_dfma_peak(ctypes.c_int(local), ctypes.c_int(2048), ctypes.c_int(5), ctypes.byref(tf), ctypes.byref(msb))
                 if rcmb == 0:
-                    dfma = {"tflops": tf.value, "ms": msb.value, "what": "148*8 blocks x 256 threads x 8 independent DFMA chains (libahmc_microbench.so)"}
+                    dfma = {"tflops": tf.value, "ms": msb.value, "what": "8 blocks per SM x 256 threads x 8 independent DFMA chains (libahmc_microbench.so)"}
 
     # ---- the path's one exchange (SURVEY 8e), inside the driver-run line: pooled warm-up on the C4 shape (funnel D=100,
     # 4096 chains per GPU, NUTS).  Per iteration, on ONE stream and with no host synchronisation: NUTS transition (K3) ->
@@ -653,9 +649,7 @@ def run_ours(args):
     fp64_ops = units_per_step * 2 * 2  # 2 DFMA per step*dim on the fast path
     roofline = {
         "bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
-        # dram__bytes_read.sum + dram__bytes_write.sum of this kernel at this shape, per launch, from the committed
-        # `ncu --set full` capture of this round (profiles/r02/k1_headline_dram.json; null when no capture is committed)
-        "traffic": measured_traffic(), "peak_source": peak_src, "kernel": "leapfrog_kernel<DIAG_GAUSS,DIAG,G=32,E=4>",
+        "peak_source": peak_src, "kernel": "leapfrog_kernel<DIAG_GAUSS,DIAG,G=32,E=4>",
         "kernel_ms": kernel_ms,
         "model": "SURVEY 8d streaming contract: (48+24/D) B per step*dim x N*D*L units per launch; the fused L-step "
                  "kernel keeps state in registers, so its COMPULSORY traffic is 1/L of that (next keys)",
@@ -708,6 +702,14 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, z):
+    """the phase point the last timed step returned, as float64 .npy files (the state is (N, D) = Julia's D x N)"""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"theta": z.theta, "r": z.r, "lp_value": z.lp.value, "lp_gradient": z.lp.gradient, "lk_value": z.lk.value}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().cpu().numpy().astype(np.float64))
+
+
 class StdoutToStderr:
     """Native libraries (NCCL prints its version banner) write to fd 1; the contract is ONE JSON line on stdout.
     Route fd 1 to stderr for the duration of the run and hand back a writer on the real stdout."""
@@ -735,6 +737,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the arrays the last timed step computed to DIR/<name>.npy (float64)")
     args = ap.parse_args()
     with StdoutToStderr() as out:
         args.emit = out.emit

@@ -1,5 +1,5 @@
 /*
- * ahmc_b200.h -- C ABI of libahmc_b200: the B200-native (sm_100a) many-chain leapfrog / HMC / NUTS
+ * ahmc_b200.h -- C ABI of libahmc_b200: the H100-native (sm_90a) many-chain leapfrog / HMC / NUTS
  * engine that slots under AdvancedHMC.jl's `AbstractIntegrator` / `Hamiltonian` / `AbstractMetric`
  * plugin surface (see INTEGRATION.md for the Julia `ccall` shim that binds every entry point).
  *
@@ -162,7 +162,7 @@ int ahmc_model_create_callback(ahmc_ctx* ctx, int32_t D, ahmc_logp_grad_fn fn, v
  *     #define AHMC_USER_COORDWISE
  *     __device__ double ahmc_user_coord(int d, double theta_d, const double* params, double* grad_d);
  *         for targets that are a sum over coordinates: term d and its derivative (every lane evaluates its own coordinates)
- * It is compiled at run time (NVRTC, sm_100a) together with the library's own kernel sources on first use of each kernel, so
+ * It is compiled at run time (NVRTC, sm_90a) together with the library's own kernel sources on first use of each kernel, so
  * phasepoint, the fused trajectory, the static HMC transition, NUTS (MultinomialTS + GeneralisedNoUTurn) and
  * find_good_stepsize run on it exactly as on a built-in target: no host round trip per step.  params[n_params] (host) is
  * copied to the device and handed to the function; lp = c0 + the function's value.  Compilation errors come back through

@@ -2,8 +2,7 @@
 executed counts) joined with `nvdisasm -c -gi` line / inline info of the SAME build.
 Usage: python scripts/ncu_line_profile.py <source.csv> <nvdisasm -gi listing of the kernel> <kernel .cu> <device .cuh> <leaves> [inner]
 ("inner": attribute to the INNERMOST frame inside the kernel's own file instead of the outermost -- for kernels whose
- body is one big inlined call, e.g. K4's tile product)
-(The r01 capture predates the template split: rebuild that commit's ahmc_nuts.cu to a cubin first; see profiles/README.md.)"""
+ body is one big inlined call, e.g. K4's tile product)"""
 import collections
 import csv
 import re

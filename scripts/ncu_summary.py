@@ -1,4 +1,4 @@
-"""Summarise an `ncu --page raw --csv` export: one JSON object per captured launch with the numbers profiles/README.md quotes
+"""Summarise an `ncu --page raw --csv` export: one JSON object per captured launch with the headline numbers
 (duration, DRAM bytes read / written, executed warp instructions, registers, occupancy, SM-active cycles).
 Usage: python scripts/ncu_summary.py <raw.csv> [<raw.csv> ...]"""
 import csv

@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, n), n
     assert set(names) == set(A._lib.PROTOTYPES), set(names) ^ set(A._lib.PROTOTYPES)
     lib.ahmc_version.restype = ctypes.c_char_p
-    assert b"sm_100a" in lib.ahmc_version()
+    assert b"sm_90a" in lib.ahmc_version()
 
 
 def test_no_cpu_fallback_without_gpu():
@@ -207,7 +207,7 @@ def test_julia_shim_struct_field_counts_match_the_c_structs():
 
 
 def test_user_target_sources_compile_under_nvrtc_without_a_gpu():
-    """ahmc_user_source_check: the library's embedded kernel sources + a user device function compile for sm_100a (NVRTC needs
+    """ahmc_user_source_check: the library's embedded kernel sources + a user device function compile for sm_90a (NVRTC needs
     no device), for every kernel a user target can run in and for both contracts; a broken source returns the NVRTC log."""
     import ctypes as C
 

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path, called through the C ABI, against
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C ABI, against
 (i) the committed 50-digit known answers and (ii) the CPU oracle on the same seeded inputs.
 Tolerance: 1e-10 relative fp64 (BASELINE.json north_star), written out below as TOL."""
 import zlib
