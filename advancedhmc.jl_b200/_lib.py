@@ -99,6 +99,9 @@ PROTOTYPES = {
     "ahmc_nuts_adapt_sample_f64": (C.c_int, [_vp, _vp, C.POINTER(Metric), C.c_int32, C.c_int64, C.c_int32, C.c_double,
                                              C.c_int32, C.POINTER(AdaptCfg), C.POINTER(Rng), C.POINTER(PhasePoint),
                                              C.POINTER(PhasePoint), _vp, C.POINTER(Stats), C.c_uint32]),
+    "ahmc_hmc_adapt_sample_f64": (C.c_int, [_vp, _vp, C.POINTER(Metric), C.c_int32, C.c_int64, C.c_int32, C.c_int32,
+                                            C.POINTER(AdaptCfg), C.POINTER(Rng), C.POINTER(PhasePoint),
+                                            C.POINTER(PhasePoint), _vp, C.POINTER(Stats), C.c_uint32]),
     "ahmc_adapt_summary_f64": (C.c_int, [_vp, C.c_int32, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_uint32]),
     "ahmc_adapt_cov_f64": (C.c_int, [_vp, C.c_int32, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_uint32]),
     "ahmc_find_good_stepsize_f64": (C.c_int, [_vp, _vp, C.POINTER(Metric), C.c_int32, C.c_int64, C.POINTER(PhasePoint),

@@ -991,7 +991,9 @@ def sample_transitions(rng: PhiloxRNG, h: Hamiltonian, kappa: HMCKernel, z: Phas
 class VectorisedStanAdaptor:
     """`StanHMCAdaptor(WelfordVar((D, N)), NesterovDualAveraging(delta, eps::Vector))`: the reference's vectorised
     adaptors -- one dual-averaging state and one windowed variance estimator PER CHAIN (stepsize.jl:178-210,
-    massmatrix.jl:141-157, stan_adaptor.jl:13-50, 137-159).  Runs inside the NUTS launch (ahmc_nuts_adapt_sample_f64)."""
+    massmatrix.jl:141-157, stan_adaptor.jl:13-50, 137-159).  Runs inside the NUTS launch (ahmc_nuts_adapt_sample_f64)
+    or the static-HMC launch (ahmc_hmc_adapt_sample_f64).  metric_estimator: "welford" (`WelfordVar((D, N))` of the
+    positions) or "nutpie" (`NutpieVar((D, N))`, massmatrix.jl:172-250: positions and gradients)."""
     delta: float = 0.8
     adapt_metric: bool = True
     init_buffer: int = 75
@@ -1001,6 +1003,37 @@ class VectorisedStanAdaptor:
     t0: float = 10.0
     kappa: float = 0.75
     n_min: int = 10
+    metric_estimator: str = "welford"
+
+
+_ESTIMATORS = {"welford": 1, "nutpie": 2}  # ahmc_adapt_cfg.adapt_metric (AHMC_ADAPT_WELFORD / AHMC_ADAPT_NUTPIE)
+
+
+def _adapt_launch_args(h: Hamiltonian, kappa: HMCKernel, z: PhasePoint, n_transitions: int, n_adapts: int,
+                       adaptor: VectorisedStanAdaptor, keep_draws: bool, keep_eps_trace: bool, rng: PhiloxRNG):
+    """buffers and descriptors shared by the in-launch adaptive NUTS / static-HMC calls"""
+    if adaptor.adapt_metric and adaptor.metric_estimator not in _ESTIMATORS:
+        raise L.InvalidArgument(L.ERR_INVALID, f"metric_estimator must be one of {sorted(_ESTIMATORS)}")
+    N, D = z._nd()
+    host = _is_host(z.theta)
+    out = _empty_pp(z.theta, with_lk_gradient=False)
+    md, keep = h.metric._desc(D, N, z.theta)
+    e0 = step_size(kappa.tau.integrator)
+    eps = _like(z.theta, (N,))
+    if np.ndim(e0) == 0:
+        eps[...] = float(e0)
+    elif host:
+        eps[...] = np.asarray(e0, dtype=np.float64)
+    else:
+        eps.copy_(e0 if hasattr(e0, "detach") else torch.as_tensor(np.asarray(e0, dtype=np.float64)))
+    minv = _like(z.theta, (N, D)) if adaptor.adapt_metric else None
+    trace = _like(z.theta, (n_transitions, N)) if keep_eps_trace else None
+    cfg = L.AdaptCfg(n_adapts, adaptor.init_buffer, adaptor.term_buffer, adaptor.window_size, adaptor.delta, adaptor.gamma,
+                     adaptor.t0, adaptor.kappa, _ESTIMATORS[adaptor.metric_estimator] if adaptor.adapt_metric else 0,
+                     adaptor.n_min, _ptr(eps), _ptr(minv), _ptr(trace))
+    rc = L.Rng(rng.seed, rng.offset, None, None, 0, None, 0, _refresh_alpha(kappa), _temper_alpha(kappa.tau.integrator))
+    draws = _like(z.theta, (n_transitions, N, D)) if keep_draws else None
+    return N, D, host, out, md, keep, eps, minv, trace, cfg, rc, draws
 
 
 def nuts_adapt_sample(rng: PhiloxRNG, h: Hamiltonian, kappa: HMCKernel, z: PhasePoint, n_transitions: int, n_adapts: int,
@@ -1015,34 +1048,47 @@ def nuts_adapt_sample(rng: PhiloxRNG, h: Hamiltonian, kappa: HMCKernel, z: Phase
     if tau.sampler is not MultinomialTS or not isinstance(tau.termination_criterion, GeneralisedNoUTurn):
         raise L.AhmcError(L.ERR_UNSUPPORTED, "in-launch adaptation: MultinomialTS + GeneralisedNoUTurn")
     ctx = get_context(_device_of(z.theta))
-    N, D = z._nd()
-    host = _is_host(z.theta)
-    out = _empty_pp(z.theta, with_lk_gradient=False)
-    md, keep = h.metric._desc(D, N, z.theta)
-    e0 = step_size(tau.integrator)
-    eps = _like(z.theta, (N,))
-    if np.ndim(e0) == 0:
-        eps[...] = float(e0)
-    elif host:
-        eps[...] = np.asarray(e0, dtype=np.float64)
-    else:
-        eps.copy_(e0 if hasattr(e0, "detach") else torch.as_tensor(np.asarray(e0, dtype=np.float64)))
-    minv = _like(z.theta, (N, D)) if adaptor.adapt_metric else None
-    trace = _like(z.theta, (n_transitions, N)) if keep_eps_trace else None
-    cfg = L.AdaptCfg(n_adapts, adaptor.init_buffer, adaptor.term_buffer, adaptor.window_size, adaptor.delta, adaptor.gamma,
-                     adaptor.t0, adaptor.kappa, 1 if adaptor.adapt_metric else 0, adaptor.n_min, _ptr(eps), _ptr(minv),
-                     _ptr(trace))
-    rc = L.Rng(rng.seed, rng.offset, None, None, 0, None, 0, _refresh_alpha(kappa), _temper_alpha(kappa.tau.integrator))
+    N, D, host, out, md, keep, eps, minv, trace, cfg, rc, draws = _adapt_launch_args(
+        h, kappa, z, n_transitions, n_adapts, adaptor, keep_draws, keep_eps_trace, rng)
     rng.offset += n_transitions
     tc = tau.termination_criterion
     st, sc = _stats_buffers(z.theta, N, True, T=n_transitions)
-    draws = _like(z.theta, (n_transitions, N, D)) if keep_draws else None
     fl = flags | (L.FLAG_HOST_BUFFERS if host else 0)
     _sync_torch(z.theta)
     zc, oc = z._c(False), out._c(False)
     ctx.check(ctx.lib.ahmc_nuts_adapt_sample_f64(ctx.h, h.target.handle(ctx), C.byref(md), D, N, tc.max_depth, tc.delta_max,
                                                  n_transitions, C.byref(cfg), C.byref(rc), C.byref(zc), C.byref(oc),
                                                  _ptr(draws), C.byref(sc), fl))
+    return out, draws, st, eps, minv, trace
+
+
+def hmc_adapt_sample(rng: PhiloxRNG, h: Hamiltonian, kappa: HMCKernel, z: PhasePoint, n_transitions: int, n_adapts: int,
+                     adaptor: VectorisedStanAdaptor, keep_draws: bool = True, keep_eps_trace: bool = False, flags: int = 0):
+    """`nuts_adapt_sample` for static HMC (`Trajectory{EndPointTS}(Leapfrog | TemperedLeapfrog, FixedNSteps(n))`): n_adapts
+    adapting + (n_transitions - n_adapts) sampling transitions per chain in ONE launch (ahmc_hmc_adapt_sample_f64), each
+    chain's dual averaging fed by its own acceptance rate min(1, exp(H0 - H')).  Same return tuple:
+    (z_last, draws | None, stats of (T, N) arrays, eps (N,), Minv (N, D) | None, eps_trace (T, N) | None)."""
+    if not isinstance(rng, PhiloxRNG):
+        raise L.InvalidArgument(L.ERR_INVALID, "in-launch adaptation draws from the on-device Philox streams")
+    tau = kappa.tau
+    if isinstance(tau.termination_criterion, FixedIntegrationTime):
+        raise L.AhmcError(L.ERR_UNSUPPORTED, "in-launch adaptation of static HMC needs FixedNSteps: with a per-chain step size "
+                                              "FixedIntegrationTime (HMCDA) has no common number of steps; use adaptation.sample")
+    if tau.sampler is not EndPointTS or not isinstance(tau.termination_criterion, FixedNSteps):
+        raise L.AhmcError(L.ERR_UNSUPPORTED, "in-launch adaptation of static HMC: EndPointTS + FixedNSteps")
+    if type(tau.integrator) not in (Leapfrog, TemperedLeapfrog):
+        raise L.AhmcError(L.ERR_UNSUPPORTED, "in-launch adaptation of static HMC runs Leapfrog / TemperedLeapfrog")
+    ctx = get_context(_device_of(z.theta))
+    N, D, host, out, md, keep, eps, minv, trace, cfg, rc, draws = _adapt_launch_args(
+        h, kappa, z, n_transitions, n_adapts, adaptor, keep_draws, keep_eps_trace, rng)
+    rng.offset += n_transitions
+    st, sc = _stats_buffers(z.theta, N, False, T=n_transitions)
+    fl = flags | (L.FLAG_HOST_BUFFERS if host else 0)
+    _sync_torch(z.theta)
+    zc, oc = z._c(False), out._c(False)
+    ctx.check(ctx.lib.ahmc_hmc_adapt_sample_f64(ctx.h, h.target.handle(ctx), C.byref(md), D, N, nsteps(tau), n_transitions,
+                                                C.byref(cfg), C.byref(rc), C.byref(zc), C.byref(oc), _ptr(draws),
+                                                C.byref(sc), fl))
     return out, draws, st, eps, minv, trace
 
 

@@ -18,6 +18,7 @@
 #define AHMC_PIPE_CE_CHUNKS 2
 #define AHMC_PIPE_DIRECT_OCC 1  // resident CTAs per SM of a direct-access launch (0 = no cap)
 
+#include "ahmc_chain_adapt.cuh"
 #include "ahmc_kernels.cuh"
 
 using namespace ahmc;
@@ -614,7 +615,7 @@ int ahmc_model_create_user(ahmc_ctx* ctx, int32_t D, const char* cuda_src, const
 }
 
 int ahmc_user_source_check(const char* cuda_src, int32_t kernel, int32_t metric_kind, int32_t D, char* log, int64_t log_len) {
-    if (!cuda_src || kernel < 0 || kernel > 4 || metric_kind < 0 || metric_kind > 2 || D < 1) return AHMC_ERR_INVALID;
+    if (!cuda_src || kernel < 0 || kernel > UK_HMC_ADAPT || metric_kind < 0 || metric_kind > 2 || D < 1) return AHMC_ERR_INVALID;
     int rc = user_source_check(cuda_src, kernel, metric_kind, D, log, log_len > 0 ? (size_t)log_len : 0);
     return rc == 0 ? AHMC_OK : (rc == -3 ? AHMC_ERR_UNSUPPORTED : AHMC_ERR_INVALID);
 }
@@ -1205,12 +1206,79 @@ static int stage_rng(Stager& st, const ahmc_rng* r, int32_t D, int64_t N, bool n
     return AHMC_OK;
 }
 
+// ---- in-launch adaptation (ahmc_nuts_adapt_sample_f64, ahmc_hmc_adapt_sample_f64): the cfg checks after the metric /
+// sampler family checks of each entry point, the staging of the adaptors' buffers, and the per-chain workspace
+static int check_adapt_cfg(ahmc_ctx* ctx, const ahmc_adapt_cfg* cfg, const ahmc_rng* rng, int32_t n_transitions) {
+    if (rng->normal_tape || rng->exp_tape || rng->dir_tape)
+        return fail(ctx, AHMC_ERR_INVALID, "in-launch adaptation draws from the Philox streams (no tapes)");
+    if (cfg->n_adapts < 0 || cfg->n_adapts > n_transitions)
+        return fail(ctx, AHMC_ERR_INVALID, "need 0 <= n_adapts <= n_transitions");
+    if (!cfg->eps_chain) return fail(ctx, AHMC_ERR_INVALID, "cfg.eps_chain (N, in/out) is required");
+    if (cfg->adapt_metric < AHMC_ADAPT_STEPSIZE || cfg->adapt_metric > AHMC_ADAPT_NUTPIE)
+        return fail(ctx, AHMC_ERR_INVALID, "cfg.adapt_metric must be AHMC_ADAPT_STEPSIZE (0), AHMC_ADAPT_WELFORD (1) or AHMC_ADAPT_NUTPIE (2)");
+    if (cfg->adapt_metric && !cfg->Minv_chain)
+        return fail(ctx, AHMC_ERR_INVALID, "cfg.Minv_chain (N x D, out) is required with adapt_metric");
+    if (cfg->init_buffer < 0 || cfg->term_buffer < 0 || cfg->window_size < 1)
+        return fail(ctx, AHMC_ERR_INVALID, "need init_buffer >= 0, term_buffer >= 0, window_size >= 1");
+    if (!(cfg->gamma > 0.0) || !(cfg->t0 >= 0.0) || !(cfg->delta > 0.0 && cfg->delta < 1.0))
+        return fail(ctx, AHMC_ERR_INVALID, "need gamma > 0, t0 >= 0, 0 < delta < 1");
+    return AHMC_OK;
+}
+static void reserve_adapt(Stager& st, const ahmc_adapt_cfg* cfg, int32_t D, int64_t N, int32_t n_transitions) {
+    st.reserve((size_t)N * 8);
+    if (cfg->Minv_chain) st.reserve((size_t)N * D * 8);
+    if (cfg->eps_trace) st.reserve((size_t)N * n_transitions * 8);
+}
+// fills `ad` (schedule, constants, staged eps / M^-1 / trace buffers); *eps_chain = the per-chain step sizes the kernel reads
+static int stage_adapt(ahmc_ctx* ctx, Stager& st, const ahmc_adapt_cfg* cfg, int32_t D, int64_t N, int32_t n_transitions,
+                       AdaptDev* ad, const double** eps_chain) {
+    ad->enabled = 1;
+    ad->n_adapts = cfg->n_adapts;
+    ad->delta = cfg->delta;
+    ad->gamma = cfg->gamma;
+    ad->t0 = cfg->t0;
+    ad->kappa = cfg->kappa;
+    ad->adapt_metric = cfg->adapt_metric;
+    ad->n_min = cfg->n_min > 0 ? cfg->n_min : 10;
+    if (!stan_window_schedule(*ad, cfg->init_buffer, cfg->term_buffer, cfg->window_size, cfg->n_adapts))
+        return fail(ctx, AHMC_ERR_UNSUPPORTED, "the window schedule (stan_adaptor.jl:13-50) needs more than %d splits",
+                    (int)(sizeof(ad->splits) / sizeof(ad->splits[0])));
+    int rc;
+    if ((rc = st.inout(cfg->eps_chain, (size_t)N, &ad->eps))) return rc;
+    *eps_chain = ad->eps;
+    if ((rc = st.out(cfg->Minv_chain, (size_t)N * D, &ad->minv))) return rc;
+    if ((rc = st.out(cfg->eps_trace, (size_t)N * n_transitions, &ad->eps_trace))) return rc;
+    return AHMC_OK;
+}
+// the context's per-chain workspace (NUTS trees, in-launch adaptors' estimators): at least `need` bytes
+static int chain_workspace(ahmc_ctx* ctx, size_t need, double** out) {
+    if (need > ctx->nuts_scratch_bytes) {
+        CU(cudaStreamSynchronize(ctx->stream));
+        cudaFree(ctx->nuts_scratch);
+        ctx->nuts_scratch = nullptr;
+        ctx->nuts_scratch_bytes = 0;
+        cudaError_t e = cudaMalloc((void**)&ctx->nuts_scratch, need);
+        if (e != cudaSuccess) return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for the NUTS workspace failed: %s", need, cudaGetErrorString(e));
+        ctx->nuts_scratch_bytes = need;
+    }
+    *out = ctx->nuts_scratch;
+    return AHMC_OK;
+}
+
 static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, int32_t D, int64_t N,
                     double eps, const double* eps_chain, int32_t n_steps, int32_t n_transitions, const ahmc_rng* rng,
                     const ahmc_phasepoint* z_in, const ahmc_phasepoint* z_out, double* draws, const ahmc_stats* stats,
-                    uint32_t flags) {
+                    uint32_t flags, const ahmc_adapt_cfg* cfg = nullptr) {
     if (!ctx || !model || !metric || !rng) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/model/metric/rng");
     if (n_transitions < 1) return fail(ctx, AHMC_ERR_INVALID, "n_transitions must be >= 1");
+    if (cfg) {
+        if (metric->kind != AHMC_METRIC_DIAG)
+            return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation needs the Diag metric (per-chain diagonal M^-1)");
+        if (model->kind == AHMC_MODEL_CALLBACK)
+            return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation needs a device-resident target: callback (split-step) models cannot run inside one launch; express the target as CUDA source (ahmc_model_create_user)");
+        int rc = check_adapt_cfg(ctx, cfg, rng, n_transitions);
+        if (rc) return rc;
+    }
     if (n_transitions > 1 && (rng->normal_tape || rng->exp_tape))
         return fail(ctx, AHMC_ERR_INVALID, "random tapes describe ONE transition; multi-transition sampling uses the Philox streams");
     if (n_transitions > 1 && model->kind == AHMC_MODEL_CALLBACK)
@@ -1242,6 +1310,7 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
     st.reserve((size_t)D * N * 8);
     st.reserve((size_t)N * 8 * 16 * n_transitions);
     if (draws) st.reserve((size_t)D * N * n_transitions * 8);
+    if (cfg) reserve_adapt(st, cfg, D, N, n_transitions);
     if ((rc = st.prepare())) return rc;
     HmcArgs h{};
     LeapfrogArgs& a = h.lf;
@@ -1250,7 +1319,11 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
     a.D = D;
     a.N = N;
     a.eps = eps;
-    if ((rc = st.in(eps_chain, (size_t)N, &a.eps_chain))) return rc;
+    if (cfg) {
+        if ((rc = stage_adapt(ctx, st, cfg, D, N, n_transitions, &h.ad, &a.eps_chain))) return rc;
+    } else if ((rc = st.in(eps_chain, (size_t)N, &a.eps_chain))) {
+        return rc;
+    }
     a.n_steps = n_steps;
     a.fwd = 1;
     a.temper_alpha = 0.0;
@@ -1313,7 +1386,7 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
         ctx->launches += nl;
         return finish_call(ctx, st, flags);
     }
-    if (n_transitions == 1 && a.th_out != a.th_in && h.rng.partial_alpha == 0.0 && !(h.rng.temper_alpha > 0.0) && !draws &&
+    if (!cfg && n_transitions == 1 && a.th_out != a.th_in && h.rng.partial_alpha == 0.0 && !(h.rng.temper_alpha > 0.0) && !draws &&
         (model->kind == AHMC_MODEL_DENSE_GAUSS || a.metric.kind == AHMC_METRIC_DENSE)) {
         // GEMM-shaped operators: refresh -> tiled DMMA trajectory (in place on z_out) -> MH select; same semantics as
         // hmc_kernel.  (Falls through to the fused generic kernel when the tile kernel is not eligible.)
@@ -1361,6 +1434,10 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
             }
         }
     }
+    if (cfg) {  // the adaptors' estimator state: chain_adapt_vectors D-vectors per chain
+        h.scratch_stride = (long long)chain_adapt_vectors(cfg->adapt_metric) * D;
+        if ((rc = chain_workspace(ctx, (size_t)h.scratch_stride * (size_t)N * sizeof(double), &h.scratch))) return rc;
+    }
     CU(launch_hmc(h, ctx->stream, &nl));
     ctx->launches += nl;
     return finish_call(ctx, st, flags);
@@ -1377,17 +1454,8 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
             return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation needs the Diag metric (per-chain diagonal M^-1)");
         if (flags & (AHMC_FLAG_NUTS_SLICE_TS | AHMC_FLAG_NUTS_CLASSIC | AHMC_FLAG_NUTS_STRICT))
             return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation is built for MultinomialTS + GeneralisedNoUTurn");
-        if (rng->normal_tape || rng->exp_tape || rng->dir_tape)
-            return fail(ctx, AHMC_ERR_INVALID, "in-launch adaptation draws from the Philox streams (no tapes)");
-        if (cfg->n_adapts < 0 || cfg->n_adapts > n_transitions)
-            return fail(ctx, AHMC_ERR_INVALID, "need 0 <= n_adapts <= n_transitions");
-        if (!cfg->eps_chain) return fail(ctx, AHMC_ERR_INVALID, "cfg.eps_chain (N, in/out) is required");
-        if (cfg->adapt_metric && !cfg->Minv_chain)
-            return fail(ctx, AHMC_ERR_INVALID, "cfg.Minv_chain (N x D, out) is required with adapt_metric");
-        if (cfg->init_buffer < 0 || cfg->term_buffer < 0 || cfg->window_size < 1)
-            return fail(ctx, AHMC_ERR_INVALID, "need init_buffer >= 0, term_buffer >= 0, window_size >= 1");
-        if (!(cfg->gamma > 0.0) || !(cfg->t0 >= 0.0) || !(cfg->delta > 0.0 && cfg->delta < 1.0))
-            return fail(ctx, AHMC_ERR_INVALID, "need gamma > 0, t0 >= 0, 0 < delta < 1");
+        int rc = check_adapt_cfg(ctx, cfg, rng, n_transitions);
+        if (rc) return rc;
     }
     if (n_transitions > 1 && (rng->normal_tape || rng->exp_tape || rng->dir_tape))
         return fail(ctx, AHMC_ERR_INVALID, "random tapes describe ONE transition; multi-transition sampling uses the Philox streams");
@@ -1406,8 +1474,8 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
         return fail(ctx, AHMC_ERR_INVALID, "AHMC_FLAG_NUTS_CLASSIC and AHMC_FLAG_NUTS_STRICT are mutually exclusive");
     if (model->kind == AHMC_MODEL_CALLBACK)
         return fail(ctx, AHMC_ERR_UNSUPPORTED, "NUTS needs a device-resident target: callback (split-step) models are supported by ahmc_leapfrog_f64 / ahmc_hmc_transition_f64 / ahmc_phasepoint_f64 only; express the target as CUDA source (ahmc_model_create_user) to run NUTS on it");
-    if (model->kind == AHMC_MODEL_USER && (cfg || (flags & (AHMC_FLAG_NUTS_SLICE_TS | AHMC_FLAG_NUTS_CLASSIC | AHMC_FLAG_NUTS_STRICT))))
-        return fail(ctx, AHMC_ERR_UNSUPPORTED, "run-time compiled targets: MultinomialTS + GeneralisedNoUTurn without in-launch adaptation");
+    if (model->kind == AHMC_MODEL_USER && (flags & (AHMC_FLAG_NUTS_SLICE_TS | AHMC_FLAG_NUTS_CLASSIC | AHMC_FLAG_NUTS_STRICT)))
+        return fail(ctx, AHMC_ERR_UNSUPPORTED, "run-time compiled targets: MultinomialTS + GeneralisedNoUTurn only");
     if (metric->kind == AHMC_METRIC_DENSE && !metric->cholU && !(flags & AHMC_FLAG_NO_REFRESH))
         return fail(ctx, AHMC_ERR_INVALID, "Dense metric needs cholU for the momentum refresh (metric.jl:311-320)");
     if (z_out->lk_gradient)
@@ -1426,11 +1494,7 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
     if (draws) st.reserve((size_t)D * N * n_transitions * 8);
     if (rng->exp_tape) st.reserve((size_t)rng->exp_stride * N * 8);
     if (rng->dir_tape) st.reserve((size_t)rng->dir_stride * N);
-    if (cfg) {
-        st.reserve((size_t)N * 8);
-        if (cfg->Minv_chain) st.reserve((size_t)N * D * 8);
-        if (cfg->eps_trace) st.reserve((size_t)N * n_transitions * 8);
-    }
+    if (cfg) reserve_adapt(st, cfg, D, N, n_transitions);
     if ((rc = st.prepare())) return rc;
     NutsArgs a{};
     a.model = model_dev(model);
@@ -1463,22 +1527,7 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
     a.N = N;
     a.eps = eps;
     if (cfg) {
-        AdaptDev& ad = a.ad;
-        ad.enabled = 1;
-        ad.n_adapts = cfg->n_adapts;
-        ad.delta = cfg->delta;
-        ad.gamma = cfg->gamma;
-        ad.t0 = cfg->t0;
-        ad.kappa = cfg->kappa;
-        ad.adapt_metric = cfg->adapt_metric ? 1 : 0;
-        ad.n_min = cfg->n_min > 0 ? cfg->n_min : 10;
-        if (!stan_window_schedule(ad, cfg->init_buffer, cfg->term_buffer, cfg->window_size, cfg->n_adapts))
-            return fail(ctx, AHMC_ERR_UNSUPPORTED, "the window schedule (stan_adaptor.jl:13-50) needs more than %d splits",
-                        (int)(sizeof(ad.splits) / sizeof(ad.splits[0])));
-        if ((rc = st.inout(cfg->eps_chain, (size_t)N, &ad.eps))) return rc;
-        a.eps_chain = ad.eps;
-        if ((rc = st.out(cfg->Minv_chain, (size_t)N * D, &ad.minv))) return rc;
-        if ((rc = st.out(cfg->eps_trace, (size_t)N * n_transitions, &ad.eps_trace))) return rc;
+        if ((rc = stage_adapt(ctx, st, cfg, D, N, n_transitions, &a.ad, &a.eps_chain))) return rc;
     } else if ((rc = st.in(eps_chain, (size_t)N, &a.eps_chain))) {
         return rc;
     }
@@ -1504,18 +1553,8 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
     if ((rc = st.out(draws, (size_t)D * N * n_transitions, &a.draws))) return rc;
     a.n_transitions = n_transitions;
     // per-chain tree workspace
-    a.scratch_stride = nuts_scratch_doubles_per_chain(D, max_depth, cfg != nullptr);
-    size_t need = (size_t)a.scratch_stride * (size_t)N * sizeof(double);
-    if (need > ctx->nuts_scratch_bytes) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->nuts_scratch);
-        ctx->nuts_scratch = nullptr;
-        ctx->nuts_scratch_bytes = 0;
-        cudaError_t e = cudaMalloc((void**)&ctx->nuts_scratch, need);
-        if (e != cudaSuccess) return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for the NUTS workspace failed: %s", need, cudaGetErrorString(e));
-        ctx->nuts_scratch_bytes = need;
-    }
-    a.scratch = ctx->nuts_scratch;
+    a.scratch_stride = nuts_scratch_doubles_per_chain(D, max_depth, cfg ? chain_adapt_vectors(cfg->adapt_metric) : 0);
+    if ((rc = chain_workspace(ctx, (size_t)a.scratch_stride * (size_t)N * sizeof(double), &a.scratch))) return rc;
     int nl = 0;
     CU(launch_nuts(a, ctx->stream, &nl));
     ctx->launches += nl;
@@ -1671,6 +1710,14 @@ int ahmc_nuts_adapt_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahm
     if (!cfg) return fail(ctx, AHMC_ERR_INVALID, "NULL cfg");
     return nuts_impl(ctx, model, metric, D, N, 0.0, nullptr, max_depth, delta_max, n_transitions, rng, z_in, z_out, draws,
                      stats, flags, cfg);
+}
+
+int ahmc_hmc_adapt_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, int32_t D, int64_t N,
+                              int32_t n_steps, int32_t n_transitions, const ahmc_adapt_cfg* cfg, const ahmc_rng* rng,
+                              const ahmc_phasepoint* z_in, const ahmc_phasepoint* z_out, double* draws,
+                              const ahmc_stats* stats, uint32_t flags) {
+    if (!cfg) return fail(ctx, AHMC_ERR_INVALID, "NULL cfg");
+    return hmc_impl(ctx, model, metric, D, N, 0.0, nullptr, n_steps, n_transitions, rng, z_in, z_out, draws, stats, flags, cfg);
 }
 
 // ---------------------------------------------------------------------------------------------- adaptor stats

@@ -85,16 +85,8 @@ struct RngDev {
     double temper_alpha;   // > 0: the transition integrates with TemperedLeapfrog(eps, alpha) (integrator.jl:174-209)
 };
 
-struct HmcArgs {
-    LeapfrogArgs lf;  // th_in/r_in/g_in/lp_in = current phase point; outputs = new phase point
-    RngDev rng;
-    StatsDev st;          // arrays of n_transitions x N entries (transition-major)
-    int refresh;          // 1: draw new momentum
-    int n_transitions;    // >= 1: persistent sampling loop inside the kernel (sampler.jl:182 `for i in 1:n_samples`)
-    double* draws;        // nullable: n_transitions x (D x N) positions, draw t of chain c at (t*N + c)*D
-};
-
-// in-kernel per-chain adaptation (K3 adaptive family): NesterovDualAveraging + windowed WelfordVar per chain
+// in-kernel per-chain adaptation (adaptive K2 / K3 forms, ahmc_chain_adapt.cuh): NesterovDualAveraging + a windowed
+// WelfordVar or NutpieVar per chain
 struct AdaptDev {
     int enabled;
     int n_adapts;                  // iterations 1..n_adapts adapt (sampler.jl:72-90)
@@ -102,7 +94,7 @@ struct AdaptDev {
     int n_splits;
     int splits[12];
     double delta, gamma, t0, kappa;  // stepsize.jl:162-172
-    int adapt_metric;                // 0: step size only
+    int adapt_metric;                // AHMC_ADAPT_STEPSIZE / _WELFORD / _NUTPIE
     int n_min;                       // massmatrix.jl:103-107
     double* eps;                     // N, out: adapted step size per chain (in: a.eps_chain / a.eps)
     double* minv;                    // N*D, out: adapted diagonal M^-1 per chain (nullable when !adapt_metric)
@@ -126,6 +118,23 @@ inline bool stan_window_schedule(AdaptDev& ad, int init_buffer, int term_buffer,
     if (ad.n_splits > 0 && ad.splits[ad.n_splits - 1] == n_adapts) --ad.n_splits;  // "avoid updating in the end"
     return true;
 }
+
+// the compiled estimator form (ahmc_chain_adapt.cuh) an adaptive launch needs: NutpieVar has its own, step size only and
+// WelfordVar share one
+inline int adapt_form(const AdaptDev& ad) { return ad.adapt_metric == AHMC_ADAPT_NUTPIE ? AHMC_ADAPT_NUTPIE : AHMC_ADAPT_WELFORD; }
+
+struct HmcArgs {
+    LeapfrogArgs lf;  // th_in/r_in/g_in/lp_in = current phase point; outputs = new phase point
+    RngDev rng;
+    StatsDev st;          // arrays of n_transitions x N entries (transition-major)
+    int refresh;          // 1: draw new momentum
+    int n_transitions;    // >= 1: persistent sampling loop inside the kernel (sampler.jl:182 `for i in 1:n_samples`)
+    double* draws;        // nullable: n_transitions x (D x N) positions, draw t of chain c at (t*N + c)*D
+    // adaptive form only (ad.enabled): the per-chain adaptors and their estimator workspace
+    AdaptDev ad;
+    double* scratch;
+    long long scratch_stride;  // doubles per chain
+};
 
 struct NutsArgs {
     ModelDev model;
@@ -274,7 +283,7 @@ bool bigd_supported(int model_kind, int metric_kind);
 cudaError_t launch_leapfrog_big(const LeapfrogArgs& a, cudaStream_t st);
 cudaError_t launch_phasepoint_big(const PhasepointArgs& a, cudaStream_t st);
 cudaError_t launch_nuts(const NutsArgs& a, cudaStream_t stream, int* n_launches);
-long long nuts_scratch_doubles_per_chain(int D, int max_depth, bool adaptive);
+long long nuts_scratch_doubles_per_chain(int D, int max_depth, int adapt_vectors);  // + adapt_vectors D-vectors
 cudaError_t launch_trajectory(const TrajArgs& a, cudaStream_t stream, int* n_launches);
 cudaError_t launch_multinomial(const MultinomialArgs& a, cudaStream_t stream, int* n_launches);
 cudaError_t launch_kick_drift(const SplitArgs& a, cudaStream_t stream, int* n_launches);
@@ -306,13 +315,14 @@ int nccl_comm_destroy(void* comm);
 int nccl_allgather_f64(const double* send, double* recv, size_t count, void* comm, cudaStream_t st);
 
 // user targets compiled at run time (ahmc_user.cu): NVRTC + the driver API, both bound with dlopen
-enum UserKernel { UK_PHASEPOINT = 0, UK_LEAPFROG = 1, UK_HMC = 2, UK_NUTS = 3, UK_FIND_EPS = 4 };
+enum UserKernel { UK_PHASEPOINT = 0, UK_LEAPFROG = 1, UK_HMC = 2, UK_NUTS = 3, UK_FIND_EPS = 4, UK_NUTS_ADAPT = 5, UK_HMC_ADAPT = 6 };
 struct UserModule;  // per-model cache of compiled kernels
 UserModule* user_module_create(const char* cuda_src, char* err, size_t err_len);
 void user_module_destroy(UserModule* m);
 // compile (first use) and launch kernel `which` of the user module for (metric, G, E); args = the kernel's argument block
+// form: the estimator form of an adaptive kernel (UK_NUTS_ADAPT / UK_HMC_ADAPT: adapt_form(ad)), 0 for the others
 cudaError_t user_launch(UserModule* m, int which, int metric_kind, int G, int E, const void* args, unsigned blocks, size_t smem,
-                        cudaStream_t st);
+                        cudaStream_t st, int form = 0);
 const char* user_last_error(const UserModule* m);
 int user_source_check(const char* cuda_src, int which, int metric_kind, int D, char* log, size_t log_len);
 const char* user_thread_error();  // message of the last failed user_launch on this thread ("" if none)

@@ -23,6 +23,7 @@
 #ifndef __CUDACC_RTC__
 #include <cstdlib>
 #endif
+#include "ahmc_chain_adapt.cuh"
 #include "ahmc_kernels.cuh"
 #include "ahmc_traj.cuh"
 
@@ -46,6 +47,7 @@ bool pick_layout(int D, int* G, int* E) {
 template <int G, int E, bool CONTIG = false>
 struct StepIO {
     static constexpr bool kContig = CONTIG;
+    static constexpr bool kChainMinv = false;
     const LeapfrogArgs& a;
     long long chain;
     int l;
@@ -132,7 +134,9 @@ __global__ void __launch_bounds__(kBlockThreads, min_blocks_lf<MODEL, METRIC, E>
 // ---------------------------------------------------------------------------------------------
 // K2: one static-HMC transition (sampler.jl:48-58 + trajectory.jl:271-300, 312-340, 863-880)
 // ---------------------------------------------------------------------------------------------
-template <int METRIC, int G, int E>
+// ADAPT: the chain adapts its own step size and diagonal M^-1 inside the launch (minv: its current M^-1, alpha: the
+// acceptance statistic of the transition just made, for dual averaging)
+template <int METRIC, int G, int E, bool ADAPT = false>
 struct HmcIO {
     const HmcArgs& h;
     long long chain;
@@ -142,8 +146,11 @@ struct HmcIO {
     long long stat_idx;    // t*N + chain
     double H0, lp0, lk0, ex;
     double r0[E];
+    double minv[ADAPT ? E : 1];
+    mutable double alpha;
 
     static constexpr bool kContig = false;
+    static constexpr bool kChainMinv = ADAPT;
     __device__ __forceinline__ bool has_g() const { return true; }
     __device__ __forceinline__ void init(double (&th)[E], double (&r)[E], double (&g)[E]) const {
         vload_nc<G, E>(th, src_th, l, h.lf.D);
@@ -202,13 +209,15 @@ struct HmcIO {
             if (st.hamiltonian_energy_error) st.hamiltonian_energy_error[stat_idx] = H - H0;
             if (st.numerical_error) st.numerical_error[stat_idx] = finite_d(H1) ? 0 : 1;
         }
+        this->alpha = alpha;
         (void)dr;
     }
 };
 
 // One launch = n_transitions static-HMC transitions per chain (the reference's `for i in 1:n_samples` loop,
-// sampler.jl:182, without adaptation): state is re-read from the output phase point, which stays L2-resident.
-template <int MODEL, int METRIC, int G, int E>
+// sampler.jl:182): state is re-read from the output phase point, which stays L2-resident.  ADAPT != 0 (the adaptor's estimator form, ahmc_chain_adapt.cuh): iterations
+// 1..n_adapts also run the chain's own StanHMCAdaptor (ahmc_chain_adapt.cuh) on its acceptance rate and draw.
+template <int MODEL, int METRIC, int G, int E, int ADAPT = 0>
 __global__ void __launch_bounds__(kBlockThreads, min_blocks_hmc<MODEL, METRIC, E>()) hmc_kernel(const HmcArgs h) {
     extern __shared__ double smem[];
     const LeapfrogArgs& a = h.lf;
@@ -219,11 +228,16 @@ __global__ void __launch_bounds__(kBlockThreads, min_blocks_hmc<MODEL, METRIC, E
     const long long chain = valid ? chain0 : a.N - 1;
     const int D = a.D;
     double* xs = smem + (size_t)grp_in_block * slab_vectors<MODEL>() * D;
-    const double eps = a.eps_chain ? __ldg(a.eps_chain + chain) : a.eps;
+    double eps = a.eps_chain ? __ldg(a.eps_chain + chain) : a.eps;
 
     MetricOps<METRIC, G, E> me;
     me.load(a.metric, chain, l, D);
-    HmcIO<METRIC, G, E> io{h, chain, l};
+    HmcIO<METRIC, G, E, (ADAPT != 0)> io{h, chain, l};
+    ChainAdapt<G, E, ADAPT == AHMC_ADAPT_NUTPIE ? AHMC_ADAPT_NUTPIE : AHMC_ADAPT_WELFORD> cad{};
+    if constexpr (ADAPT) {
+        __syncwarp();  // every lane has read its starting eps (ad.eps) before lane 0 writes it back
+        if (valid) cad.begin(h.ad, h.scratch + h.scratch_stride * chain, eps, me.Minv, chain, l, D);
+    }
     for (int t = 0; t < h.n_transitions; ++t) {
         const bool first = (t == 0);
         io.src_th = first ? a.th_in + a.ld_in * chain : a.th_out + a.ld_out * chain;
@@ -256,7 +270,16 @@ __global__ void __launch_bounds__(kBlockThreads, min_blocks_hmc<MODEL, METRIC, E
         io.lp0 = map_nonfinite(first ? a.lp_in[chain] : a.lp_out[chain]);
         io.H0 = -(io.lp0 + io.lk0);
         io.ex = h.rng.exp_tape ? h.rng.exp_tape[chain] : philox_exp(h.rng.seed, off, chain, 0);
+        if constexpr (ADAPT) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) io.minv[e] = me.Minv[e];
+        }
         run_trajectory<MODEL, METRIC, G, E>(a.model, a.metric, D, chain, valid, l, xs, eps, a.n_steps, h.rng.temper_alpha, a.flags, io);
+        if constexpr (ADAPT) {  // iteration t + 1 of `sample` (sampler.jl:182)
+            if (valid)
+                cad.update(h.ad, h.scratch + h.scratch_stride * chain, t + 1, io.stat_idx, io.alpha, a.th_out + a.ld_out * chain, a.g_out + a.ld_out * chain, eps, me.Minv,
+                           chain, l, D);
+        }
         __syncwarp();
     }
 }
@@ -595,18 +618,22 @@ static cudaError_t launch_pp_t(const PhasepointArgs& a, cudaStream_t st) {
     phasepoint_kernel<MODEL, METRIC, G, E><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
     return cudaGetLastError();
 }
-template <int MODEL, int METRIC, int G, int E>
+template <int MODEL, int METRIC, int G, int E, int ADAPT = 0>
 static cudaError_t launch_hmc_t(const HmcArgs& a, cudaStream_t st) {
     const int chains_per_block = kBlockThreads / G;
     const long long blocks = (a.lf.N + chains_per_block - 1) / chains_per_block;
     size_t sm = smem_bytes(MODEL, METRIC, a.lf.D, G);
     if (sm > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(hmc_kernel<MODEL, METRIC, G, E>,
+        cudaError_t e = cudaFuncSetAttribute(hmc_kernel<MODEL, METRIC, G, E, ADAPT>,
                                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
         if (e != cudaSuccess) return e;
     }
-    hmc_kernel<MODEL, METRIC, G, E><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
+    hmc_kernel<MODEL, METRIC, G, E, ADAPT><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
     return cudaGetLastError();
+}
+template <int FORM, int MODEL, int METRIC, int G, int E>
+static cudaError_t launch_hmc_adapt_t(const HmcArgs& a, cudaStream_t st) {
+    return launch_hmc_t<MODEL, METRIC, G, E, FORM>(a, st);
 }
 template <int METRIC, int G, int E>
 static cudaError_t launch_kd_t(const SplitArgs& a, cudaStream_t st) {
@@ -672,6 +699,20 @@ static cudaError_t pp_layout(const PhasepointArgs& a, cudaStream_t st, int G, in
 template <int MODEL, int METRIC>
 static cudaError_t hmc_layout(const HmcArgs& a, cudaStream_t st, int G, int E) {
     AHMC_DISPATCH_LAYOUT(launch_hmc_t, MODEL, METRIC);
+}
+template <int MODEL, int FORM>
+static cudaError_t hmc_adapt_layout(const HmcArgs& a, cudaStream_t st, int G, int E) {
+    AHMC_DISPATCH_LAYOUT(launch_hmc_adapt_t, FORM, MODEL, AHMC_METRIC_DIAG);
+}
+template <int FORM>
+static cudaError_t hmc_adapt_model(const HmcArgs& a, cudaStream_t st, int G, int E) {
+    switch (a.lf.model.kind) {
+        case AHMC_MODEL_STD_NORMAL: return hmc_adapt_layout<AHMC_MODEL_STD_NORMAL, FORM>(a, st, G, E);
+        case AHMC_MODEL_DIAG_GAUSS: return hmc_adapt_layout<AHMC_MODEL_DIAG_GAUSS, FORM>(a, st, G, E);
+        case AHMC_MODEL_DENSE_GAUSS: return hmc_adapt_layout<AHMC_MODEL_DENSE_GAUSS, FORM>(a, st, G, E);
+        case AHMC_MODEL_FUNNEL: return hmc_adapt_layout<AHMC_MODEL_FUNNEL, FORM>(a, st, G, E);
+    }
+    return cudaErrorInvalidValue;
 }
 template <int METRIC>
 static cudaError_t kd_layout(const SplitArgs& a, cudaStream_t st, int G, int E) {
@@ -759,8 +800,14 @@ cudaError_t launch_hmc(const HmcArgs& a, cudaStream_t st, int* n_launches) {
     if (n_launches) *n_launches += 1;
     if (a.lf.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
         const int cpb = kBlockThreads / G;
-        return user_launch((UserModule*)a.lf.model.user, UK_HMC, a.lf.metric.kind, G, E, &a, (unsigned)((a.lf.N + cpb - 1) / cpb),
-                           smem_bytes(AHMC_MODEL_USER, a.lf.metric.kind, a.lf.D, G), st);
+        return user_launch((UserModule*)a.lf.model.user, a.ad.enabled ? UK_HMC_ADAPT : UK_HMC, a.lf.metric.kind, G, E, &a,
+                           (unsigned)((a.lf.N + cpb - 1) / cpb), smem_bytes(AHMC_MODEL_USER, a.lf.metric.kind, a.lf.D, G), st,
+                           a.ad.enabled ? adapt_form(a.ad) : 0);
+    }
+    if (a.ad.enabled) {  // the adaptive form: Diag metric only (the chain adapts its diagonal M^-1)
+        if (a.lf.metric.kind != AHMC_METRIC_DIAG) return cudaErrorInvalidValue;
+        return adapt_form(a.ad) == AHMC_ADAPT_NUTPIE ? hmc_adapt_model<AHMC_ADAPT_NUTPIE>(a, st, G, E)
+                                                     : hmc_adapt_model<AHMC_ADAPT_WELFORD>(a, st, G, E);
     }
     AHMC_DISPATCH_MM(hmc_layout, a.lf.model.kind, a.lf.metric.kind);
 }

@@ -4,8 +4,8 @@
 
 namespace ahmc {
 
-long long nuts_scratch_doubles_per_chain(int D, int max_depth, bool adaptive) {
-    return nuts_level_doubles(D, max_depth) + (adaptive ? 2LL * D : 0);
+long long nuts_scratch_doubles_per_chain(int D, int max_depth, int adapt_vectors) {
+    return nuts_level_doubles(D, max_depth) + (long long)adapt_vectors * D;
 }
 
 // A (D x D, column-major) -> columns of leading dimension coop_lds(D), rows >= D zero: what the cooperative products stream
@@ -24,18 +24,21 @@ cudaError_t launch_pad_columns(const double* A, int D, double* out, cudaStream_t
 
 cudaError_t launch_nuts_variants(const NutsArgs& a, cudaStream_t st);  // ahmc_nuts_var.cu
 cudaError_t launch_nuts_adaptive(const NutsArgs& a, cudaStream_t st);  // ahmc_nuts_adapt.cu
+cudaError_t launch_nuts_nutpie(const NutsArgs& a, cudaStream_t st);    // ahmc_nuts_nutpie.cu
 
 cudaError_t launch_nuts(const NutsArgs& a, cudaStream_t st, int* n_launches) {
     if (n_launches) *n_launches += 1;
-    if (a.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernel of a user target (default family only, ahmc_user.cu)
+    if (a.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernel of a user target (default / adaptive family, ahmc_user.cu)
         int G, E;
-        if (!pick_layout(a.D, &G, &E) || a.ad.enabled || a.sampler != 0 || a.criterion != 0) return cudaErrorInvalidValue;
+        if (!pick_layout(a.D, &G, &E) || a.sampler != 0 || a.criterion != 0) return cudaErrorInvalidValue;
+        if (a.ad.enabled && a.metric.kind != AHMC_METRIC_DIAG) return cudaErrorInvalidValue;
         const int cpb = kBlockThreads / G;
         const int maxd = a.max_depth > 0 ? a.max_depth : 1;
         const size_t sm = smem_bytes(AHMC_MODEL_USER, a.metric.kind, a.D, G) + (size_t)cpb * maxd * kLevelScalars * sizeof(double);
-        return user_launch((UserModule*)a.model.user, UK_NUTS, a.metric.kind, G, E, &a, (unsigned)((a.N + cpb - 1) / cpb), sm, st);
+        return user_launch((UserModule*)a.model.user, a.ad.enabled ? UK_NUTS_ADAPT : UK_NUTS, a.metric.kind, G, E, &a,
+                           (unsigned)((a.N + cpb - 1) / cpb), sm, st, a.ad.enabled ? adapt_form(a.ad) : 0);
     }
-    if (a.ad.enabled) return launch_nuts_adaptive(a, st);
+    if (a.ad.enabled) return a.ad.adapt_metric == AHMC_ADAPT_NUTPIE ? launch_nuts_nutpie(a, st) : launch_nuts_adaptive(a, st);
     if (a.sampler != 0 || a.criterion != 0) return launch_nuts_variants(a, st);
     return nuts_dispatch<false, false, false>(a, st);
 }

@@ -24,7 +24,7 @@
 // (ahmc_nuts.cu), the SliceTS / Classic / Strict variants (ahmc_nuts_var.cu), and the form that adapts step size and
 // diagonal metric per chain inside the launch (ahmc_nuts_adapt.cu).
 #pragma once
-#include "ahmc_kernels.cuh"
+#include "ahmc_chain_adapt.cuh"
 
 namespace ahmc {
 
@@ -33,7 +33,7 @@ namespace ahmc {
 // becomes an edge) | per level k (7 vectors): 0 rho, 1 rfirst, 2 cand theta, 3 cand r, 4 cand g, 5 rlast (Strict),
 // 6 theta_first (Classic)
 constexpr int kLevelVecs = 7;
-// (+ 2 vectors at the end for the in-kernel Welford state of the adaptive form: mean, M2)
+// (+ chain_adapt_vectors(adapt_metric) vectors at the end for the estimator state of the adaptive form, ahmc_chain_adapt.cuh)
 __host__ __device__ inline long long nuts_level_doubles(int D, int max_depth) {
     return (long long)(9 + kLevelVecs * (max_depth > 0 ? max_depth : 1)) * D;
 }
@@ -72,6 +72,9 @@ constexpr int nuts_min_blocks() { return E <= 4 ? 3 : (E <= 8 ? 2 : 1); }
 // SliceTS (trajectory.jl:102-109,144-145,164-166,178-189,202,500-502) and the Classic / StrictGeneralised criteria
 // (trajectory.jl:551-557, 579-613), selected at run time by a.sampler / a.criterion.
 //
+// ADAPT = 0: no adaptation; else the estimator form of the chain's in-launch adaptor (ahmc_chain_adapt.cuh):
+// AHMC_ADAPT_WELFORD (step size only or WelfordVar, by a.ad.adapt_metric) or AHMC_ADAPT_NUTPIE.
+//
 // COOP = true (dense operators, one chain per warp, default family): the block has kCoopWarps warps and every D x D product
 // (dH/dr with a Dense metric, grad lp of a dense Gaussian) is a CTA-wide rendezvous -- the matrix is streamed from L2 into
 // shared memory once per BLOCK and each element feeds kCoopWarps FMAs (matvec_coop, ahmc_device.cuh) instead of every warp
@@ -79,7 +82,7 @@ constexpr int nuts_min_blocks() { return E <= 4 ? 3 : (E <= 8 ? 2 : 1); }
 // All warps of a block must then reach the product sites together: the votes that steer the loop around them are block-wide,
 // and a warp whose chain is idle or finished keeps taking part (its results are ignored, like idle groups of a warp).
 // (the tile flag must not be called FULL: that is the namespace's all-lanes mask used by every *_sync below)
-template <int MODEL, int METRIC, int G, int E, bool VAR, bool ADAPT, bool FULLTILE, bool COOP = false>
+template <int MODEL, int METRIC, int G, int E, bool VAR, int ADAPT, bool FULLTILE, bool COOP = false>
 __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 : nuts_min_blocks<E>()) nuts_kernel(const NutsArgs a) {
     static_assert(!COOP || (G == 32 && !VAR), "COOP: one chain per warp, default family");
     constexpr int kThreads = COOP ? kCoopThreads : kBlockThreads;
@@ -126,11 +129,9 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
     auto level = [&](int k) { return base + (9 + kLevelVecs * (long long)k) * D; };
 
     double eps_c = a.eps_chain ? __ldg(a.eps_chain + chain) : a.eps;
-    // adaptive family: per-chain dual-averaging state (all lanes of the group hold the same values) and the chain's
-    // Welford accumulators (mean, M2 per coordinate, owned lane-wise) behind the tree workspace
-    double da_mu = 0.0, da_xbar = 0.0, da_Hbar = 0.0, da_m = 0.0, w_n = 0.0;
-    double* W_MU = base + nuts_level_doubles(D, a.max_depth);
-    double* W_M2 = W_MU + D;
+    // adaptive family: the chain's adaptor (ahmc_chain_adapt.cuh), its estimator state behind the tree workspace
+    ChainAdapt<G, E, ADAPT == AHMC_ADAPT_NUTPIE ? AHMC_ADAPT_NUTPIE : AHMC_ADAPT_WELFORD> cad{};
+    auto cad_ws = [&]() { return base + nuts_level_doubles(D, a.max_depth); };
 
     ModelOps<MODEL, G, E> mo;
     MetricOps<METRIC, G, E> me;
@@ -277,17 +278,7 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
                 vstore<G, E>(a.th_out + a.ld_out * chain, s.th, l, D);
                 vstore<G, E>(a.r_out + a.ld_out * chain, s.r, l, D);
                 vstore<G, E>(a.g_out + a.ld_out * chain, s.g, l, D);
-                if (ADAPT && first) {  // DAState(eps) (stepsize.jl:27-36); WelfordVar zeros (massmatrix.jl:109-118)
-                    da_mu = log(10.0 * eps_c);
-                    da_xbar = da_Hbar = da_m = w_n = 0.0;
-                    double zero[E];
-#pragma unroll
-                    for (int e = 0; e < E; ++e) zero[e] = 0.0;
-                    vstore<G, E>(W_MU, zero, l, D);
-                    vstore<G, E>(W_M2, zero, l, D);
-                    if (a.ad.minv) vstore<G, E>(a.ad.minv + (long long)D * chain, me.Minv, l, D);
-                    if (l == 0) a.ad.eps[chain] = eps_c;
-                }
+                if (ADAPT && first) cad.begin(a.ad, cad_ws(), eps_c, me.Minv, chain, l, D);
                 lw_tree = 0.0;
                 ww_tree = 1.0;
                 if (VAR && samp == 1) {  // SliceTS(rng, z0) = SliceTS(z0, neg_energy(z0) - randexp(rng), 1) (:144-145)
@@ -335,66 +326,9 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
                     if (st.tree_depth) st.tree_depth[si] = j;
                     if (st.numerical_error) st.numerical_error[si] = term_num ? 1 : 0;
                 }
-                if (ADAPT) {
-                    const int it = t + 1;  // 1-based iteration of `sample` (sampler.jl:182)
-                    if (a.ad.eps_trace && l == 0) a.ad.eps_trace[si] = eps_c;
-                    if (it <= a.ad.n_adapts) {
-                        // adapt_stepsize! (stepsize.jl:178-210), one chain: alpha = this transition's acceptance rate
-                        const double alpha = sa_tree / (double)na_tree;
-                        const double amin = (alpha != alpha) ? alpha : (alpha < 1.0 ? alpha : 1.0);  // min(1, alpha)
-                        const double m1 = da_m + 1.0;
-                        const double eta_H = 1.0 / (m1 + a.ad.t0);
-                        const double Hn = (1.0 - eta_H) * da_Hbar + eta_H * (a.ad.delta - amin);
-                        const double x = da_mu - Hn * (sqrt(m1) / a.ad.gamma);
-                        const double eta_x = pow(m1, -a.ad.kappa);
-                        const double xn = (1.0 - eta_x) * da_xbar + eta_x * x;
-                        const double en = exp(x);
-                        if (finite_d(en)) {  // else the previous state stays (stepsize.jl:199-203, per chain)
-                            da_m = m1;
-                            da_Hbar = Hn;
-                            da_xbar = xn;
-                            eps_c = en;
-                        }
-                        bool split = false;  // is_window_end (stan_adaptor.jl:135)
-                        for (int q = 0; q < a.ad.n_splits; ++q) split = split || (a.ad.splits[q] == it);
-                        if (a.ad.adapt_metric && it >= a.ad.window_start && it <= a.ad.window_end) {
-                            // push!(::WelfordVar, theta) (massmatrix.jl:141-149) with the new draw
-                            double th_new[E], wmu[E], wm2[E];
-                            vload_nc<G, E>(th_new, a.th_out + a.ld_out * chain, l, D);
-                            vload_nc<G, E>(wmu, W_MU, l, D);
-                            vload_nc<G, E>(wm2, W_M2, l, D);
-                            w_n += 1.0;
-                            const double f = (w_n - 1.0) / w_n;
-#pragma unroll
-                            for (int e = 0; e < E; ++e) {
-                                const double dl = th_new[e] - wmu[e];
-                                wmu[e] = wmu[e] + dl / w_n;
-                                wm2[e] = wm2[e] + dl * dl * f;
-                            }
-                            if (split && w_n >= (double)a.ad.n_min) {  // update! + get_estimation (massmatrix.jl:60-62, 152-157)
-                                const double c1 = w_n / ((w_n + 5.0) * (w_n - 1.0)), c2 = 1e-3 * (5.0 / (w_n + 5.0));
-#pragma unroll
-                                for (int e = 0; e < E; ++e) me.Minv[e] = (l + G * e < D) ? c1 * wm2[e] + c2 : 0.0;
-                                vstore<G, E>(a.ad.minv + (long long)D * chain, me.Minv, l, D);
-                            }
-                            vstore<G, E>(W_MU, wmu, l, D);
-                            vstore<G, E>(W_M2, wm2, l, D);
-                        }
-                        if (split) {  // reset!(ssa); reset!(pc) (stan_adaptor.jl:155-158; stepsize.jl:38-52)
-                            da_m = 0.0;
-                            da_mu = log(10.0 * eps_c);
-                            da_xbar = da_Hbar = 0.0;
-                            w_n = 0.0;
-                            double zero[E];
-#pragma unroll
-                            for (int e = 0; e < E; ++e) zero[e] = 0.0;
-                            vstore<G, E>(W_MU, zero, l, D);
-                            vstore<G, E>(W_M2, zero, l, D);
-                        }
-                        if (it == a.ad.n_adapts) eps_c = exp(da_xbar);  // finalize! (stepsize.jl:54-62)
-                        if (l == 0) a.ad.eps[chain] = eps_c;
-                    }
-                }
+                if constexpr (ADAPT)  // iteration t + 1 of `sample` (sampler.jl:182): alpha = this transition's acceptance rate
+                    cad.update(a.ad, cad_ws(), t + 1, si, sa_tree / (double)na_tree, a.th_out + a.ld_out * chain, a.g_out + a.ld_out * chain,
+                               eps_c, me.Minv, chain, l, D);
                 ++t;
                 if (t < a.n_transitions) need_init = true;
                 else finished = true;
@@ -797,7 +731,7 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
 }
 
 #if !defined(AHMC_SIMT_EMULATION) && !defined(__CUDACC_RTC__)  // host launch code (skipped by the CPU SIMT emulation harness and by NVRTC)
-template <int MODEL, int METRIC, int G, int E, bool VAR, bool ADAPT>
+template <int MODEL, int METRIC, int G, int E, bool VAR, int ADAPT>
 static cudaError_t launch_nuts_v(const NutsArgs& a, cudaStream_t st) {
     const int maxd = a.max_depth > 0 ? a.max_depth : 1;
     constexpr bool kDenseOps = MODEL == AHMC_MODEL_DENSE_GAUSS || METRIC == AHMC_METRIC_DENSE;
@@ -842,7 +776,7 @@ static cudaError_t launch_nuts_v(const NutsArgs& a, cudaStream_t st) {
     }
 }
 
-template <int MODEL, int METRIC, bool VAR, bool ADAPT>
+template <int MODEL, int METRIC, bool VAR, int ADAPT>
 static cudaError_t nuts_layout(const NutsArgs& a, cudaStream_t st, int G, int E) {
     if (G == 4 && E == 1) return launch_nuts_v<MODEL, METRIC, 4, 1, VAR, ADAPT>(a, st);
     if (G == 8 && E == 1) return launch_nuts_v<MODEL, METRIC, 8, 1, VAR, ADAPT>(a, st);
@@ -855,8 +789,8 @@ static cudaError_t nuts_layout(const NutsArgs& a, cudaStream_t st, int G, int E)
     return cudaErrorInvalidValue;
 }
 
-// model x metric dispatch of one (VAR, ADAPT) family; DIAG_ONLY restricts the family to the Diag metric
-template <bool VAR, bool ADAPT, bool DIAG_ONLY>
+// model x metric dispatch of one (VAR, ADAPT) family (ADAPT: 0, or the adaptor's estimator form, ahmc_chain_adapt.cuh); DIAG_ONLY restricts the family to the Diag metric
+template <bool VAR, int ADAPT, bool DIAG_ONLY>
 static cudaError_t nuts_dispatch(const NutsArgs& a, cudaStream_t st) {
     int G, E;
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;

@@ -27,6 +27,9 @@
 //    bool has_g()                                                 -- false: init() leaves g unset, recompute it from theta
 //    static constexpr bool kContig                                -- true: the fast path uses init_c / done_c, the same
 //                                                                    calls on lane-contiguous vectors (ahmc_device.cuh)
+//    static constexpr bool kChainMinv                             -- true: a Diag metric's M^-1 is the functor's register
+//                                                                    vector minv[E] (a chain adapting its own metric inside
+//                                                                    the launch), not `metric.Minv`
 // `done` is called exactly once per valid chain, by all lanes of the chain's group.
 #pragma once
 #include "ahmc_device.cuh"
@@ -61,7 +64,14 @@ __device__ __forceinline__ void run_trajectory(const ModelDev& model, const Metr
                 if constexpr (C) f.init_c(x, r, g0);
                 else f.init(x, r, g0);
                 const bool have_g = f.has_g();
-                if constexpr (METRIC == AHMC_METRIC_DIAG) lload<C, G, E>(mi, metric.Minv + metric.chain_stride * chain, l, D);
+                if constexpr (METRIC == AHMC_METRIC_DIAG) {
+                    if constexpr (F::kChainMinv) {
+#pragma unroll
+                        for (int e = 0; e < E; ++e) mi[e] = f.minv[e];
+                    } else {
+                        lload<C, G, E>(mi, metric.Minv + metric.chain_stride * chain, l, D);
+                    }
+                }
                 if constexpr (MODEL == AHMC_MODEL_DIAG_GAUSS) {
                     lload<C, G, E>(wi, model.p1, l, D);
                     lload<C, G, E>(mu, model.p0, l, D);
@@ -157,6 +167,10 @@ __device__ __forceinline__ void run_trajectory(const ModelDev& model, const Metr
     MetricOps<METRIC, G, E> me;
     mo.load(model, l, D);
     me.load(metric, chain, l, D);
+    if constexpr (F::kChainMinv) {
+#pragma unroll
+        for (int e = 0; e < E; ++e) me.Minv[e] = f.minv[e];
+    }
     ChainState<E> s;
     f.init(s.th, s.r, s.g);
     if (!f.has_g()) mo.eval(s.th, s.g, xs, l);  // no cached gradient handed over: dH/dtheta at the start point

@@ -3,8 +3,8 @@
 // The reference calls an arbitrary Julia closure per leapfrog step; a persistent CUDA loop cannot call back into the host.
 // A target expressible as a CUDA device function is therefore compiled at run time TOGETHER with the kernel sources
 // (NVRTC; the sources are embedded in the library at build time, ahmc_embedded_sources.cu) and the resulting kernels --
-// phasepoint, the fused trajectory (K1), the static transition (K2), NUTS (K3, default family), find_good_stepsize -- are
-// the same code as the built-in targets with ModelOps<AHMC_MODEL_USER>::eval calling the user's function.  One instantiation
+// phasepoint, the fused trajectory (K1), the static transition (K2), NUTS (K3, default family), find_good_stepsize and the
+// adaptive forms of K2 and K3 (in-launch warm-up, ahmc_chain_adapt.cuh) -- are the same code as the built-in targets with ModelOps<AHMC_MODEL_USER>::eval calling the user's function.  One instantiation
 // (kernel x metric x layout) is compiled on first use and cached in the model.  NVRTC and the driver API are bound with
 // dlopen: the library loads without them and fails loudly (AHMC_ERR_UNSUPPORTED) when a user target is requested.
 #include <dlfcn.h>
@@ -115,7 +115,7 @@ struct UserModule {
         void* fn = nullptr;
         size_t smem_set = 0;
     };
-    std::map<long long, Fn> fns;  // key = which | metric << 4 | G << 8 | E << 16
+    std::map<long long, Fn> fns;  // key = which | metric << 4 | G << 8 | E << 16 | form << 24
 };
 
 UserModule* user_module_create(const char* cuda_src, char* err, size_t err_len) {
@@ -141,7 +141,7 @@ const char* user_thread_error() { return t_user_err.c_str(); }
 void user_thread_error_clear() { t_user_err.clear(); }
 
 // compile kernel `which` of the user target; load it when `out` is given (needs a device), else only check that it compiles
-static bool compile(UserModule* m, int which, int metric, int G, int E, UserModule::Fn* out) {
+static bool compile(UserModule* m, int which, int metric, int G, int E, int form, UserModule::Fn* out) {
     char expr[160];
     const char* unit = "ahmc_leapfrog.cu";
     switch (which) {
@@ -149,8 +149,11 @@ static bool compile(UserModule* m, int which, int metric, int G, int E, UserModu
         case UK_LEAPFROG: snprintf(expr, sizeof expr, "ahmc::leapfrog_kernel<%d, %d, %d, %d, false>", AHMC_MODEL_USER, metric, G, E); break;
         case UK_HMC: snprintf(expr, sizeof expr, "ahmc::hmc_kernel<%d, %d, %d, %d>", AHMC_MODEL_USER, metric, G, E); break;
         case UK_FIND_EPS: snprintf(expr, sizeof expr, "ahmc::find_eps_kernel<%d, %d, %d, %d>", AHMC_MODEL_USER, metric, G, E); break;
+        case UK_HMC_ADAPT: snprintf(expr, sizeof expr, "ahmc::hmc_kernel<%d, %d, %d, %d, %d>", AHMC_MODEL_USER, metric, G, E, form); break;
         case UK_NUTS:
-            snprintf(expr, sizeof expr, "ahmc::nuts_kernel<%d, %d, %d, %d, false, false, false>", AHMC_MODEL_USER, metric, G, E);
+        case UK_NUTS_ADAPT:
+            snprintf(expr, sizeof expr, "ahmc::nuts_kernel<%d, %d, %d, %d, false, %d, false>", AHMC_MODEL_USER, metric, G, E,
+                     which == UK_NUTS_ADAPT ? form : 0);
             unit = "ahmc_nuts_kernel.cuh";
             break;
         default: m->err = "unknown kernel"; return false;
@@ -207,13 +210,14 @@ static bool compile(UserModule* m, int which, int metric, int G, int E, UserModu
 }
 
 cudaError_t user_launch(UserModule* m, int which, int metric_kind, int G, int E, const void* args, unsigned blocks, size_t smem,
-                        cudaStream_t st) {
+                        cudaStream_t st, int form) {
     if (!m) return cudaErrorInvalidValue;
-    const long long key = (long long)which | ((long long)metric_kind << 4) | ((long long)G << 8) | ((long long)E << 16);
+    const long long key =
+        (long long)which | ((long long)metric_kind << 4) | ((long long)G << 8) | ((long long)E << 16) | ((long long)form << 24);
     auto it = m->fns.find(key);
     if (it == m->fns.end()) {
         UserModule::Fn f;
-        if (!compile(m, which, metric_kind, G, E, &f)) {
+        if (!compile(m, which, metric_kind, G, E, form, &f)) {
             t_user_err = m->err;
             return cudaErrorInvalidSource;
         }
@@ -247,9 +251,16 @@ int user_source_check(const char* cuda_src, int which, int metric_kind, int D, c
     if (!pick_layout(D, &G, &E)) return -1;
     UserModule m;
     m.src = cuda_src;
-    if (compile(&m, which, metric_kind, G, E, nullptr)) return 0;
-    if (log) snprintf(log, log_len, "%s", m.err.c_str());
-    return -1;
+    // the adaptive kernels: both estimator forms
+    const bool adaptive = which == UK_NUTS_ADAPT || which == UK_HMC_ADAPT;
+    for (int form : {adaptive ? AHMC_ADAPT_WELFORD : 0, adaptive ? AHMC_ADAPT_NUTPIE : 0}) {
+        if (!compile(&m, which, metric_kind, G, E, form, nullptr)) {
+            if (log) snprintf(log, log_len, "%s", m.err.c_str());
+            return -1;
+        }
+        if (!adaptive) break;
+    }
+    return 0;
 }
 
 }  // namespace ahmc

@@ -170,7 +170,8 @@ int ahmc_model_create_callback(ahmc_ctx* ctx, int32_t D, ahmc_logp_grad_fn fn, v
 int ahmc_model_create_user(ahmc_ctx* ctx, int32_t D, const char* cuda_src, const double* params, int32_t n_params, double c0,
                            ahmc_model** out);
 /* Compile-only check of a user target (no device, no context needed): kernel 0 phasepoint, 1 trajectory, 2 static HMC,
- * 3 NUTS, 4 find_good_stepsize; the layout follows from D.  AHMC_OK, or AHMC_ERR_INVALID with the NVRTC log in `log`. */
+ * 3 NUTS, 4 find_good_stepsize, 5 NUTS with in-launch adaptation (ahmc_nuts_adapt_sample_f64), 6 static HMC with in-launch
+ * adaptation (ahmc_hmc_adapt_sample_f64); the layout follows from D.  AHMC_OK, or AHMC_ERR_INVALID with the NVRTC log in `log`. */
 int ahmc_user_source_check(const char* cuda_src, int32_t kernel, int32_t metric_kind, int32_t D, char* log, int64_t log_len);
 int ahmc_model_destroy(ahmc_ctx* ctx, ahmc_model* model);
 
@@ -251,8 +252,8 @@ int ahmc_nuts_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metr
 
 /* Warm-up + sampling in ONE launch with the reference's VECTORISED adaptors: every chain owns a
  * `NesterovDualAveraging` state (src/adaptation/stepsize.jl:178-210: eps is a length-N vector and adapts per chain) and,
- * with adapt_metric, a windowed `WelfordVar` over its own draws (massmatrix.jl:141-157 with a D x N variance, i.e. a
- * per-chain diagonal M^-1), scheduled like `StanHMCAdaptor` (stan_adaptor.jl:13-50, 137-159: windows, reset of both
+ * with adapt_metric, a windowed `WelfordVar` or `NutpieVar` over its own draws (massmatrix.jl:141-157, 172-250 with a
+ * D x N variance, i.e. a per-chain diagonal M^-1), scheduled like `StanHMCAdaptor` (stan_adaptor.jl:13-50, 137-159: windows, reset of both
  * adaptors at each window end, `finalize!` eps = exp(x_bar) after iteration n_adapts).  Because nothing is pooled,
  * chains never wait for each other: iterations 1..n_adapts adapt, n_adapts+1..n_transitions sample with the final
  * eps / M^-1.  Requires the Diag metric (shared or per-chain M^-1 as the starting point), MultinomialTS +
@@ -263,16 +264,31 @@ typedef struct ahmc_adapt_cfg {
     int32_t init_buffer, term_buffer, window_size; /* Stan defaults 75 / 50 / 25; a schedule with more than 12 window
                                                       ends (tiny window_size, huge n_adapts) -> AHMC_ERR_UNSUPPORTED */
     double delta, gamma, t0, kappa;               /* 0.8, 0.05, 10, 0.75 (stepsize.jl:162-172) */
-    int32_t adapt_metric;                         /* 0: step size only; 1: + per-chain WelfordVar */
-    int32_t n_min;                                /* WelfordVar n_min, 10 (massmatrix.jl:103-107) */
+    int32_t adapt_metric;                         /* AHMC_ADAPT_STEPSIZE / _WELFORD / _NUTPIE; other values: AHMC_ERR_INVALID */
+    int32_t n_min;                                /* estimator n_min, 10 (massmatrix.jl:103-107) */
     double* eps_chain;  /* N, in: initial step size per chain; out: adapted step size per chain */
-    double* Minv_chain; /* N x D, out: adapted diagonal M^-1 per chain (required iff adapt_metric) */
+    double* Minv_chain; /* N x D, out: adapted diagonal M^-1 per chain (required iff adapt_metric != 0) */
     double* eps_trace;  /* nullable, n_transitions x N: the step size each transition used (`step_size` stat) */
 } ahmc_adapt_cfg;
+/* ahmc_adapt_cfg.adapt_metric: the per-chain metric estimator */
+#define AHMC_ADAPT_STEPSIZE 0 /* step size only: M^-1 stays the metric's */
+#define AHMC_ADAPT_WELFORD 1  /* WelfordVar((D, N)) of the positions (massmatrix.jl:141-157) */
+#define AHMC_ADAPT_NUTPIE 2   /* NutpieVar((D, N)) of positions and gradients (massmatrix.jl:172-250):
+                                 M^-1 = sqrt(var(theta) / var(grad log pi)), each variance regularised as WelfordVar's */
 int ahmc_nuts_adapt_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, int32_t D, int64_t N,
                                int32_t max_depth, double delta_max, int32_t n_transitions, const ahmc_adapt_cfg* cfg,
                                const ahmc_rng* rng, const ahmc_phasepoint* z_in, const ahmc_phasepoint* z_out,
                                double* draws, const ahmc_stats* stats, uint32_t flags);
+/* The same warm-up + sampling in ONE launch for static HMC (`StanHMCAdaptor` with `HMCKernel(Trajectory{EndPointTS}(
+ * Leapfrog | TemperedLeapfrog, FixedNSteps(n_steps)))`): the persistent static-HMC loop of ahmc_hmc_sample_f64, each
+ * chain's dual averaging fed by its transition's acceptance_rate = min(1, exp(H0 - H')).  Same cfg, requirements and
+ * errors as ahmc_nuts_adapt_sample_f64 (Diag metric, Philox randomness, 0 <= n_adapts <= n_transitions); partial momentum
+ * refreshment and tempering as in ahmc_hmc_sample_f64.  n_adapts = 0 gives ahmc_hmc_sample_f64's results bit for bit.
+ * (`FixedIntegrationTime` has no in-launch form: with a per-chain eps its number of steps differs per chain.) */
+int ahmc_hmc_adapt_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, int32_t D, int64_t N,
+                              int32_t n_steps, int32_t n_transitions, const ahmc_adapt_cfg* cfg, const ahmc_rng* rng,
+                              const ahmc_phasepoint* z_in, const ahmc_phasepoint* z_out, double* draws,
+                              const ahmc_stats* stats, uint32_t flags);
 
 /* `find_good_stepsize(rng, h, theta)` (src/trajectory.jl:768-837) for N chains at once, each running its own search, in
  * ONE launch: momentum draw (rng->normal_tape or Philox), the direction probe, the crossing loop and the bisection, every

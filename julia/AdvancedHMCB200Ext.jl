@@ -487,6 +487,35 @@ function b200_sample_nuts(rng, h::Hamiltonian, lf::B200Leapfrog, tc::Generalised
     return draws, ϵ, Minv
 end
 
+"""
+`sample(rng, h, HMCKernel(Trajectory{EndPointTS}(lf, FixedNSteps(L))), θ, n_samples, adaptor, n_adapts)` with the same
+vectorised adaptors as `b200_sample_nuts`, as ONE static-HMC launch (ahmc_hmc_adapt_sample_f64).  `metric_estimator` =
+`:welford` (`WelfordVar((D, N))`) or `:nutpie` (`NutpieVar((D, N))`).  Returns (θ draws D×N×n_samples, per-chain ϵ, M⁻¹ D×N).
+"""
+function b200_sample_hmc(rng, h::Hamiltonian, lf::B200Leapfrog, n_steps::Int, θ::CuMatrix{Float64}, n_samples::Int,
+                         n_adapts::Int; δ=0.8, adapt_metric=true, metric_estimator=:welford, init_buffer=75, term_buffer=50,
+                         window_size=25)
+    D, N = size(θ)
+    z = b200_phasepoint(lf.target, h, θ, CUDA.zeros(Float64, D, N))
+    zout = fresh_pp(z)
+    ϵ = CUDA.fill(Float64(first(step_size(lf))), N); Minv = CUDA.ones(Float64, D, N)
+    draws = CUDA.zeros(Float64, D, N, n_samples)
+    α = CUDA.zeros(Float64, N * n_samples)
+    st = Ref(CStats(C_NULL, C_NULL, dptr(α), C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL))
+    am = adapt_metric ? (metric_estimator === :nutpie ? 2 : 1) : 0
+    cfg = Ref(CAdaptCfg(n_adapts, init_buffer, term_buffer, window_size, δ, 0.05, 10.0, 0.75, am, 10,
+                        dptr(ϵ), dptr(Minv), C_NULL))
+    rg = Ref(CRng(rand(rng, UInt64), 0, C_NULL, C_NULL, 0, C_NULL, 0, 0.0, 0.0))
+    md = Ref(cmetric(h.metric, N)); zi = Ref(cpp(z)); zo = Ref(cpp(zout; lk_gradient=false))
+    GC.@preserve z zout ϵ Minv draws α begin
+        check(ccall((:ahmc_hmc_adapt_sample_f64, libahmc), Cint,
+                    (Ptr{Cvoid}, Ptr{Cvoid}, Ref{CMetric}, Int32, Int64, Int32, Int32, Ref{CAdaptCfg}, Ref{CRng},
+                     Ref{CPhasePoint}, Ref{CPhasePoint}, Ptr{Float64}, Ref{CStats}, UInt32),
+                    context().h, lf.target.handle, md, D, N, n_steps, n_samples, cfg, rg, zi, zo, dptr(draws), st, 0))
+    end
+    return draws, ϵ, Minv
+end
+
 # ---- adaptor statistics and the pooled multi-GPU adaptor (src/adaptation/*.jl) -----------------------------
 "Pooled adaptor record of one iteration: [N, sum min(1,α), mean(θ), M2(θ)] (ahmc_adapt_summary_f64)."
 function b200_adapt_summary(θ::CuMatrix{Float64}, α::CuVector{Float64})
