@@ -220,13 +220,24 @@ int check_common(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metr
     }
     int G, E;
     if (!pick_layout(D, &G, &E)) {
-        // D > 512: `step` and `phasepoint` stream the chain through registers tile by tile (ahmc_bigd.cu) for the separable
+        // D > 512: the streaming form (ahmc_bigd.cu, ahmc_bigd_hmc.cu) runs `step`, `phasepoint`, `rand_momentum`, static
+        // EndPointTS transitions (one, several, with in-launch adaptation) and `find_good_stepsize` for the separable
         // targets and the funnel with Unit / Diag metrics; everything else is register-resident and stops at 512
-        if (streaming_ok && model && metric && bigd_supported(model->kind, metric->kind)) return AHMC_OK;
+        // (rand_momentum passes no model: any Unit / Diag metric streams)
+        if (streaming_ok && metric && bigd_supported(model ? model->kind : AHMC_MODEL_STD_NORMAL, metric->kind)) return AHMC_OK;
         return fail(ctx, AHMC_ERR_UNSUPPORTED,
                     "D=%d: this entry point / target / metric combination is register-resident (D <= 512); D > 512 is supported by "
-                    "ahmc_leapfrog_f64 and ahmc_phasepoint_f64 for std-normal, diagonal-Gaussian and funnel targets with Unit / Diag metrics", D);
+                    "step, phasepoint, rand_momentum, static EndPointTS transitions, sampling and in-launch adaptation, and "
+                    "find_good_stepsize, for std-normal, diagonal-Gaussian and funnel targets with Unit / Diag metrics (not NUTS, "
+                    "MultinomialTS static transitions, full trajectories, Dense metrics, dense-Gaussian, run-time compiled or "
+                    "callback targets)", D);
     }
+    return AHMC_OK;
+}
+
+// the Philox momentum draw at D > 512 indexes its blocks up to D/2 in the 24 counter bits that `offset << 24` leaves free
+int check_philox_d(ahmc_ctx* ctx, int32_t D) {
+    if (D >= (1 << 25)) return fail(ctx, AHMC_ERR_INVALID, "D=%d: Philox momentum draws need D < 2^25", D);
     return AHMC_OK;
 }
 
@@ -1148,7 +1159,8 @@ int ahmc_leapfrog_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric*
 int ahmc_rand_momentum_f64(ahmc_ctx* ctx, const ahmc_metric* metric, int32_t D, int64_t N, const ahmc_rng* rng,
                            double* r, int64_t ld, uint32_t flags) {
     if (!ctx || !metric || !rng || !r) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/metric/rng/r");
-    int rc = check_common(ctx, nullptr, metric, D, N);
+    int rc = check_common(ctx, nullptr, metric, D, N, true);
+    if (!rc && !rng->normal_tape) rc = check_philox_d(ctx, D);
     if (rc) return rc;
     if (ld < D) return fail(ctx, AHMC_ERR_INVALID, "ld < D");
     if (metric->kind == AHMC_METRIC_DENSE && !metric->cholU)
@@ -1289,7 +1301,9 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
         return fail(ctx, AHMC_ERR_INVALID, "partial_refresh_alpha must be in (-1, 1)");
     if (!(rng->temper_alpha >= 0.0) || std::isinf(rng->temper_alpha))
         return fail(ctx, AHMC_ERR_INVALID, "temper_alpha must be 0 (plain Leapfrog) or a finite alpha > 0 (TemperedLeapfrog)");
-    int rc = check_common(ctx, model, metric, D, N);
+    int rc = check_common(ctx, model, metric, D, N, true);
+    if (!rc && D > 512 && rng->temper_alpha > 0.0) rc = fail(ctx, AHMC_ERR_UNSUPPORTED, "TemperedLeapfrog at D > 512 is not built");
+    if (!rc && D > 512 && !(flags & AHMC_FLAG_NO_REFRESH) && !rng->normal_tape) rc = check_philox_d(ctx, D);
     if (rc) return rc;
     if ((rc = check_pp(ctx, z_in, D, "z_in", true, N))) return rc;
     if ((rc = check_pp(ctx, z_out, D, "z_out", true, N))) return rc;
@@ -1434,8 +1448,9 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
             }
         }
     }
-    if (cfg) {  // the adaptors' estimator state: chain_adapt_vectors D-vectors per chain
-        h.scratch_stride = (long long)chain_adapt_vectors(cfg->adapt_metric) * D;
+    if (cfg || D > 512) {  // the adaptors' estimator state: chain_adapt_vectors D-vectors per chain; at D > 512 also the
+                           // transition's start point, kBigHmcVectors D-vectors per chain ahead of it (ahmc_bigd_hmc.cu)
+        h.scratch_stride = (long long)((D > 512 ? kBigHmcVectors : 0) + (cfg ? chain_adapt_vectors(cfg->adapt_metric) : 0)) * D;
         if ((rc = chain_workspace(ctx, (size_t)h.scratch_stride * (size_t)N * sizeof(double), &h.scratch))) return rc;
     }
     CU(launch_hmc(h, ctx->stream, &nl));
@@ -1784,7 +1799,8 @@ int ahmc_find_good_stepsize_f64(ahmc_ctx* ctx, const ahmc_model* model, const ah
                                 const ahmc_phasepoint* z, const ahmc_rng* rng, double initial_step_size, int32_t max_n_iters,
                                 double* eps_out, double* r_out, uint32_t flags) {
     if (!ctx || !model || !metric || !rng || !eps_out) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/model/metric/rng/eps_out");
-    int rc = check_common(ctx, model, metric, D, N);
+    int rc = check_common(ctx, model, metric, D, N, true);
+    if (!rc && D > 512 && !rng->normal_tape) rc = check_philox_d(ctx, D);
     if (rc) return rc;
     if (!z || (N > 0 && (!z->theta || !z->lp_value || !z->lp_gradient)))
         return fail(ctx, AHMC_ERR_INVALID, "z.theta / lp_value / lp_gradient is NULL (call ahmc_phasepoint_f64 first)");
@@ -1816,6 +1832,7 @@ int ahmc_find_good_stepsize_f64(ahmc_ctx* ctx, const ahmc_model* model, const ah
     a.max_iters = max_n_iters;
     if ((rc = st.out(eps_out, (size_t)N, &a.eps_out))) return rc;
     if ((rc = st.out(r_out, cin, &a.r_out))) return rc;
+    if (D > 512 && (rc = chain_workspace(ctx, (size_t)kBigFindEpsVectors * D * (size_t)N * sizeof(double), &a.scratch))) return rc;
     int nl = 0;
     CU(launch_find_eps(a, ctx->stream, &nl));
     ctx->launches += nl;

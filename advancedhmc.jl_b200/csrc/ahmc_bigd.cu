@@ -1,102 +1,12 @@
 // ahmc_bigd.cu -- `step` and `phasepoint` for D > 512 (the reference has no bound on D, src/metric.jl:52-72): the
 // register-resident layouts of K1 stop at 512 coordinates per chain, so here a warp STREAMS its chain through registers in
-// tiles of 512 coordinates (the same 32 lanes x 16 coordinates vector ops), the state living in the output arrays (L1 / L2
-// resident between the two passes of a step).  Per leapfrog step (src/integrator.jl:235-247):
-//   pass 1 over the tiles:  r -= eps/2 g;  theta += eps dH/dr(r);  accumulate what the gradient needs from ALL of theta
-//                           (the funnel's sum over i >= 2 of theta_i^2 e^{-v});
-//   pass 2 over the tiles:  g = -grad lp(theta);  r -= eps/2 g;  accumulate lp, the kinetic energy and the isfinite test.
+// tiles of 512 coordinates, the state living in the output arrays (L1 / L2 resident between the two passes of a step).
+// The step itself is big_step (ahmc_bigd.cuh), shared with the transition and step-size kernels of ahmc_bigd_hmc.cu.
 // Targets: std-normal, diagonal Gaussian, Neal's funnel; metrics: Unit, Diag (shared or per chain).  Dense operators at
 // D > 512 need the tiled GEMM form inside a CTA-per-tile kernel and are reported as unsupported.
-#include "ahmc_kernels.cuh"
+#include "ahmc_bigd.cuh"
 
 namespace ahmc {
-
-constexpr int kBigE = 16, kBigTile = 32 * kBigE;  // coordinates per tile
-
-template <int MODEL>
-struct BigModel {
-    const double *m, *w;
-    double c0;
-    int D;
-    // per-tile contribution to the quantity the gradient needs from the whole vector (funnel: sum_{d>=1} th_d^2)
-    __device__ __forceinline__ double pre(const double (&th)[kBigE], int d0, int l) const {
-        double p = 0.0;
-        if (MODEL == AHMC_MODEL_FUNNEL) {
-#pragma unroll
-            for (int e = 0; e < kBigE; ++e) {
-                const int d = d0 + l + 32 * e;
-                if (d >= 1 && d < D) p = fma(th[e], th[e], p);
-            }
-        }
-        return p;
-    }
-    // g tile (MINUS gradient) and the tile's lp partial; v, ev, S: funnel globals (S = e^{-v} sum_{d>=1} th_d^2)
-    __device__ __forceinline__ double grad(const double (&th)[kBigE], double (&g)[kBigE], int d0, int l, double v, double ev, double S) const {
-        double part = 0.0;
-#pragma unroll
-        for (int e = 0; e < kBigE; ++e) {
-            const int d = d0 + l + 32 * e;
-            const bool in = d < D;
-            if (MODEL == AHMC_MODEL_STD_NORMAL) {
-                g[e] = in ? th[e] : 0.0;
-                part = fma(g[e], g[e], part);
-            } else if (MODEL == AHMC_MODEL_DIAG_GAUSS) {
-                const double diff = in ? th[e] - __ldg(m + d) : 0.0;
-                g[e] = in ? diff * __ldg(w + d) : 0.0;
-                part = fma(diff, g[e], part);
-            } else {  // funnel
-                if (d == 0) g[e] = v / 9.0 - (S - (double)(D - 1)) * 0.5;
-                else g[e] = in ? th[e] * ev : 0.0;
-            }
-        }
-        return part;
-    }
-    __device__ __forceinline__ double lp(double part_sum, double v, double S) const {
-        if (MODEL == AHMC_MODEL_FUNNEL) return c0 - v * v / 18.0 - (S + (double)(D - 1) * v) * 0.5;
-        return fma(-0.5, part_sum, c0);
-    }
-};
-
-__device__ __forceinline__ void tile_load(double (&x)[kBigE], const double* base, int d0, int l, int D) {
-#pragma unroll
-    for (int e = 0; e < kBigE; ++e) {
-        const int d = d0 + l + 32 * e;
-        x[e] = d < D ? base[d] : 0.0;
-    }
-}
-__device__ __forceinline__ void tile_store(double* base, const double (&x)[kBigE], int d0, int l, int D) {
-#pragma unroll
-    for (int e = 0; e < kBigE; ++e) {
-        const int d = d0 + l + 32 * e;
-        if (d < D) base[d] = x[e];
-    }
-}
-
-// gradient / lp of the chain's current theta (in `th` array, global), written to g; returns lp (all lanes) and finiteness of g
-template <int MODEL>
-__device__ __forceinline__ double big_eval(const BigModel<MODEL>& mo, const double* th, double* g, int l, int D, bool& fin) {
-    double S = 0.0, v = 0.0, ev = 0.0;
-    if (MODEL == AHMC_MODEL_FUNNEL) {
-        for (int d0 = 0; d0 < D; d0 += kBigTile) {
-            double t[kBigE];
-            tile_load(t, th, d0, l, D);
-            S += mo.pre(t, d0, l);
-        }
-        v = th[0];
-        ev = exp(-v);
-        S = Grp<32>::sum(S) * ev;
-    }
-    double part = 0.0;
-    for (int d0 = 0; d0 < D; d0 += kBigTile) {
-        double t[kBigE], gg[kBigE];
-        tile_load(t, th, d0, l, D);
-        part += mo.grad(t, gg, d0, l, v, ev, S);
-#pragma unroll
-        for (int e = 0; e < kBigE; ++e) fin = fin && finite_d(gg[e]);
-        tile_store(g, gg, d0, l, D);
-    }
-    return mo.lp(Grp<32>::sum(part), v, S);
-}
 
 template <int MODEL, int METRIC>
 __global__ void __launch_bounds__(kBlockThreads) leapfrog_big_kernel(const LeapfrogArgs a) {
@@ -108,7 +18,6 @@ __global__ void __launch_bounds__(kBlockThreads) leapfrog_big_kernel(const Leapf
     const int D = a.D;
     double eps = a.eps_chain ? __ldg(a.eps_chain + chain) : a.eps;
     eps = a.fwd ? eps : -eps;  // integrator.jl:226
-    const double he = 0.5 * eps;
     BigModel<MODEL> mo{a.model.p0, a.model.p1, a.model.c0, D};
     const double* Mi = METRIC == AHMC_METRIC_DIAG ? a.metric.Minv + a.metric.chain_stride * chain : nullptr;
     double* th = a.th_out + a.ld_out * chain;
@@ -128,66 +37,14 @@ __global__ void __launch_bounds__(kBlockThreads) leapfrog_big_kernel(const Leapf
     double lp = 0.0, lk = 0.0;
     int steps = 0;
     fin = true;
+    double* dr = a.dr_out ? a.dr_out + a.ld_out * chain : nullptr;
     for (int i = 1; i <= a.n_steps; ++i) {
-        // pass 1: half kick with the cached gradient, drift
-        double S = 0.0;
-        for (int d0 = 0; d0 < D; d0 += kBigTile) {
-            double t[kBigE], rr[kBigE], gg[kBigE];
-            tile_load(t, th, d0, l, D);
-            tile_load(rr, r, d0, l, D);
-            tile_load(gg, g, d0, l, D);
-#pragma unroll
-            for (int e = 0; e < kBigE; ++e) {
-                const int d = d0 + l + 32 * e;
-                rr[e] = fma(-he, gg[e], rr[e]);
-                const double dr = METRIC == AHMC_METRIC_DIAG ? (d < D ? __ldg(Mi + d) : 0.0) * rr[e] : rr[e];
-                t[e] = fma(eps, dr, t[e]);
-            }
-            S += mo.pre(t, d0, l);
-            tile_store(th, t, d0, l, D);
-            tile_store(r, rr, d0, l, D);
-        }
-        __syncwarp();
-        double v = 0.0, ev = 0.0;
-        if (MODEL == AHMC_MODEL_FUNNEL) {
-            v = th[0];
-            ev = exp(-v);
-            S = Grp<32>::sum(S) * ev;
-        }
-        // pass 2: gradient at the new position, second half kick, energies, isfinite(z) (hamiltonian.jl:141-142)
-        double lp_part = 0.0, lk_part = 0.0;
-        bool f = true;
-        const bool last = (i == a.n_steps);
-        for (int d0 = 0; d0 < D; d0 += kBigTile) {
-            double t[kBigE], rr[kBigE], gg[kBigE], dr[kBigE];
-            tile_load(t, th, d0, l, D);
-            tile_load(rr, r, d0, l, D);
-            lp_part += mo.grad(t, gg, d0, l, v, ev, S);
-#pragma unroll
-            for (int e = 0; e < kBigE; ++e) {
-                const int d = d0 + l + 32 * e;
-                rr[e] = fma(-he, gg[e], rr[e]);
-                const double mi = METRIC == AHMC_METRIC_DIAG ? (d < D ? __ldg(Mi + d) : 0.0) : 1.0;
-                dr[e] = mi * rr[e];
-                lk_part = METRIC == AHMC_METRIC_DIAG ? fma(rr[e] * rr[e], mi, lk_part) : fma(rr[e], rr[e], lk_part);
-                f = f && finite_d(gg[e]) && finite_d(dr[e]);
-            }
-            tile_store(r, rr, d0, l, D);
-            tile_store(g, gg, d0, l, D);
-            if (a.dr_out) tile_store(a.dr_out + a.ld_out * chain, dr, d0, l, D);
-        }
-        __syncwarp();
-        lp = mo.lp(Grp<32>::sum(lp_part), v, S);
-        lk = -0.5 * Grp<32>::sum(lk_part);
-        f = Grp<32>::all(f) && finite_d(lp) && finite_d(lk);
-        lp = map_nonfinite(lp);
-        lk = map_nonfinite(lk);
+        const bool f = big_step<MODEL, METRIC>(mo, Mi, eps, th, r, g, dr, l, D, lp, lk);
         steps = i;
         if (!f) {  // the non-finite phase point is what is returned (integrator.jl:252-258)
             fin = false;
             break;
         }
-        (void)last;
     }
     if (l == 0) {
         a.lp_out[chain] = lp;
@@ -233,23 +90,6 @@ bool bigd_supported(int model_kind, int metric_kind) {
            (metric_kind == AHMC_METRIC_UNIT || metric_kind == AHMC_METRIC_DIAG);
 }
 
-#define AHMC_BIG_DISPATCH(KERNEL, model_kind, metric_kind, ...)                                                      \
-    do {                                                                                                             \
-        const bool diag = (metric_kind) == AHMC_METRIC_DIAG;                                                         \
-        switch (model_kind) {                                                                                        \
-            case AHMC_MODEL_STD_NORMAL:                                                                              \
-                if (diag) KERNEL<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__); \
-                else KERNEL<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_UNIT><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__);      \
-                break;                                                                                               \
-            case AHMC_MODEL_DIAG_GAUSS:                                                                              \
-                if (diag) KERNEL<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__); \
-                else KERNEL<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__);      \
-                break;                                                                                               \
-            default:                                                                                                 \
-                if (diag) KERNEL<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__);     \
-                else KERNEL<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__);          \
-        }                                                                                                            \
-    } while (0)
 
 cudaError_t launch_leapfrog_big(const LeapfrogArgs& a, cudaStream_t st) {
     if (!bigd_supported(a.model.kind, a.metric.kind) || a.temper_alpha > 0.0) return cudaErrorNotSupported;

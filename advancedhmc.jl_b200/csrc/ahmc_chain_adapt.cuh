@@ -62,6 +62,37 @@ struct ChainAdapt {
         vstore<G, E>(WMU + D, wm2, l, D);
     }
 
+    // adapt_stepsize! (stepsize.jl:178-210), one chain, with acceptance statistic alpha
+    __device__ __forceinline__ void adapt_stepsize(const AdaptDev& ad, double alpha, double& eps) {
+        const double amin = (alpha != alpha) ? alpha : (alpha < 1.0 ? alpha : 1.0);  // min(1, alpha)
+        const double m1 = m + 1.0;
+        const double eta_H = 1.0 / (m1 + ad.t0);
+        const double Hn = (1.0 - eta_H) * Hbar + eta_H * (ad.delta - amin);
+        const double x = mu - Hn * (sqrt(m1) / ad.gamma);
+        const double eta_x = pow(m1, -ad.kappa);
+        const double xn = (1.0 - eta_x) * xbar + eta_x * x;
+        const double en = exp(x);
+        if (finite_d(en)) {  // else the previous state stays (stepsize.jl:199-203, per chain)
+            m = m1;
+            Hbar = Hn;
+            xbar = xn;
+            eps = en;
+        }
+    }
+    // is_window_end (stan_adaptor.jl:135)
+    static __device__ __forceinline__ bool window_end(const AdaptDev& ad, int it) {
+        bool split = false;
+        for (int q = 0; q < ad.n_splits; ++q) split = split || (ad.splits[q] == it);
+        return split;
+    }
+    // the scalar part of the reset at a window end: reset!(ssa) and the estimator's draw count
+    __device__ __forceinline__ void reset(double eps) {
+        m = 0.0;
+        mu = log(10.0 * eps);
+        xbar = Hbar = 0.0;
+        n = 0.0;
+    }
+
     // DAState(eps) and empty estimators (massmatrix.jl:109-118); reports the starting eps and M^-1
     __device__ __forceinline__ void begin(const AdaptDev& ad, double* W, double eps, const double (&minv)[E], long long chain, int l,
                                           int D) {
@@ -78,23 +109,8 @@ struct ChainAdapt {
                                            const double* g, double& eps, double (&minv)[E], long long chain, int l, int D) {
         if (ad.eps_trace && l == 0) ad.eps_trace[si] = eps;
         if (it > ad.n_adapts) return;
-        // adapt_stepsize! (stepsize.jl:178-210), one chain
-        const double amin = (alpha != alpha) ? alpha : (alpha < 1.0 ? alpha : 1.0);  // min(1, alpha)
-        const double m1 = m + 1.0;
-        const double eta_H = 1.0 / (m1 + ad.t0);
-        const double Hn = (1.0 - eta_H) * Hbar + eta_H * (ad.delta - amin);
-        const double x = mu - Hn * (sqrt(m1) / ad.gamma);
-        const double eta_x = pow(m1, -ad.kappa);
-        const double xn = (1.0 - eta_x) * xbar + eta_x * x;
-        const double en = exp(x);
-        if (finite_d(en)) {  // else the previous state stays (stepsize.jl:199-203, per chain)
-            m = m1;
-            Hbar = Hn;
-            xbar = xn;
-            eps = en;
-        }
-        bool split = false;  // is_window_end (stan_adaptor.jl:135)
-        for (int q = 0; q < ad.n_splits; ++q) split = split || (ad.splits[q] == it);
+        adapt_stepsize(ad, alpha, eps);
+        const bool split = window_end(ad, it);
         if (ad.adapt_metric && it >= ad.window_start && it <= ad.window_end) {
             if constexpr (EST == AHMC_ADAPT_NUTPIE) {
                 // NutpieVar (massmatrix.jl:235-248): positions and gradients, M^-1 = sqrt(est(theta) ./ est(gradient));
@@ -133,10 +149,7 @@ struct ChainAdapt {
             }
         }
         if (split) {  // reset!(ssa); reset!(pc) (stan_adaptor.jl:155-158; stepsize.jl:38-52)
-            m = 0.0;
-            mu = log(10.0 * eps);
-            xbar = Hbar = 0.0;
-            n = 0.0;
+            reset(eps);
             clear(ad, W, l, D);
         }
         if (it == ad.n_adapts) eps = exp(xbar);  // finalize! (stepsize.jl:54-62)

@@ -60,6 +60,7 @@ struct FindEpsArgs {
     int max_iters;
     double* eps_out;            // N
     double* r_out;              // nullable, D x N (ld): the momentum each search used
+    double* scratch;            // D > 512 only: kBigFindEpsVectors D-vectors per chain (ahmc_bigd_hmc.cu)
 };
 
 struct StatsDev {
@@ -134,6 +135,8 @@ struct HmcArgs {
     AdaptDev ad;
     double* scratch;
     long long scratch_stride;  // doubles per chain
+    // D > 512 (ahmc_bigd_hmc.cu): scratch also holds the transition's start point, kBigHmcVectors D-vectors per chain ahead
+    // of the estimator's
 };
 
 struct NutsArgs {
@@ -282,6 +285,14 @@ cudaError_t launch_pad_columns(const double* A, int D, double* out, cudaStream_t
 bool bigd_supported(int model_kind, int metric_kind);
 cudaError_t launch_leapfrog_big(const LeapfrogArgs& a, cudaStream_t st);
 cudaError_t launch_phasepoint_big(const PhasepointArgs& a, cudaStream_t st);
+// D > 512: rand_momentum, static EndPointTS transitions (plain and in-launch adaptive) and find_good_stepsize in the
+// streaming form (ahmc_bigd_hmc.cu), each with a per-chain workspace of this many D-vectors (the adaptive transition adds
+// its estimator's chain_adapt_vectors)
+constexpr int kBigHmcVectors = 3;      // the start point: theta, -grad lp, the refreshed momentum
+constexpr int kBigFindEpsVectors = 4;  // the drawn momentum and one probe's phase point (theta, r, -grad lp)
+cudaError_t launch_rand_momentum_big(const MomentumArgs& a, cudaStream_t st);
+cudaError_t launch_hmc_big(const HmcArgs& a, cudaStream_t st);
+cudaError_t launch_find_eps_big(const FindEpsArgs& a, cudaStream_t st);
 cudaError_t launch_nuts(const NutsArgs& a, cudaStream_t stream, int* n_launches);
 long long nuts_scratch_doubles_per_chain(int D, int max_depth, int adapt_vectors);  // + adapt_vectors D-vectors
 cudaError_t launch_trajectory(const TrajArgs& a, cudaStream_t stream, int* n_launches);

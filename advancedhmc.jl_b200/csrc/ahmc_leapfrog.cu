@@ -768,6 +768,10 @@ cudaError_t launch_leapfrog(const LeapfrogArgs& a, cudaStream_t st, int* n_launc
 
 cudaError_t launch_find_eps(const FindEpsArgs& a, cudaStream_t st, int* n_launches) {
     int G, E;
+    if (a.D > 512) {  // beyond the register-resident layouts: the streaming form (ahmc_bigd_hmc.cu)
+        if (n_launches) *n_launches += 1;
+        return launch_find_eps_big(a, st);
+    }
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
     if (a.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
@@ -796,6 +800,10 @@ cudaError_t launch_phasepoint(const PhasepointArgs& a, cudaStream_t st, int* n_l
 
 cudaError_t launch_hmc(const HmcArgs& a, cudaStream_t st, int* n_launches) {
     int G, E;
+    if (a.lf.D > 512) {
+        if (n_launches) *n_launches += 1;
+        return launch_hmc_big(a, st);
+    }
     if (!pick_layout(a.lf.D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
     if (a.lf.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
@@ -843,6 +851,10 @@ cudaError_t launch_mh_select(const MhArgs& a, cudaStream_t st, int* n_launches) 
 
 cudaError_t launch_rand_momentum(const MomentumArgs& a, cudaStream_t st, int* n_launches) {
     int G, E;
+    if (a.D > 512) {
+        if (n_launches) *n_launches += 1;
+        return launch_rand_momentum_big(a, st);
+    }
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
     switch (a.metric.kind) {

@@ -187,7 +187,10 @@ int ahmc_phasepoint_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metri
  *   n_steps < 0 integrates backward (integrator.jl:221-226).  temper_alpha <= 0: no tempering.
  *   status[N] / steps_done[N] may be NULL.  z_in->lp_gradient may be NULL ("not cached": recomputed on the device).
  *   D <= 512: every target x metric, chain state register-resident.  D > 512: std-normal / diagonal-Gaussian / funnel
- *   targets with Unit / Diag metrics (the chain is streamed through registers tile by tile); same for ahmc_phasepoint_f64. */
+ *   targets with Unit / Diag metrics (the chain is streamed through registers tile by tile, no TemperedLeapfrog); same for
+ *   ahmc_phasepoint_f64, and every D > 512 transition / step-size search integrates with this same step.  Beyond 512
+ *   there is no NUTS, no MultinomialTS static transition, no full trajectory, no Dense metric or dense-Gaussian target and
+ *   no run-time compiled or callback target (AHMC_ERR_UNSUPPORTED). */
 int ahmc_leapfrog_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, int32_t D, int64_t N,
                       double eps, const double* eps_chain, int32_t n_steps, double temper_alpha,
                       const ahmc_phasepoint* z_in, const ahmc_phasepoint* z_out, uint32_t* status,
@@ -202,13 +205,18 @@ int ahmc_leapfrog_trajectory_f64(ahmc_ctx* ctx, const ahmc_model* model, const a
                                  const ahmc_phasepoint* z_in, const ahmc_phasepoint* traj, int64_t step_stride,
                                  int32_t* steps_done, uint32_t flags);
 
-/* rand_momentum(rng, metric, kinetic, theta)  (src/metric.jl:290-320): r[D x N] from normals (tape or Philox). */
+/* rand_momentum(rng, metric, kinetic, theta)  (src/metric.jl:290-320): r[D x N] from normals (tape or Philox).
+ * Unit and Diag metrics at any D; Dense at D <= 512.  The Philox normal of (seed, offset, chain, coordinate d) does not
+ * depend on D: the first 512 coordinates of a D > 512 draw are the D = 512 draw.  Philox draws need D < 2^25. */
 int ahmc_rand_momentum_f64(ahmc_ctx* ctx, const ahmc_metric* metric, int32_t D, int64_t N, const ahmc_rng* rng,
                            double* r, int64_t ld, uint32_t flags);
 
 /* One static-HMC transition for all chains: refresh (src/sampler.jl:48-58, hamiltonian.jl:213-220) +
  * `transition(rng, h, Trajectory{EndPointTS,...,FixedNSteps}, z)` (src/trajectory.jl:271-300,336-340)
- * + `mh_accept_ratio` (:863-880) + `accept_phasepoint!` (:312-332) + momentum flip (:283). */
+ * + `mh_accept_ratio` (:863-880) + `accept_phasepoint!` (:312-332) + momentum flip (:283).
+ * D > 512: the combinations of ahmc_leapfrog_f64's streaming form, without TemperedLeapfrog (the same for
+ * ahmc_hmc_sample_f64, ahmc_hmc_adapt_sample_f64 and ahmc_find_good_stepsize_f64); the start point is kept in a
+ * context-owned workspace of 3 D-vectors per chain, so z_out may alias z_in.  NUTS stops at D = 512. */
 int ahmc_hmc_transition_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, int32_t D, int64_t N,
                             double eps, const double* eps_chain, int32_t n_steps, const ahmc_rng* rng,
                             const ahmc_phasepoint* z_in, const ahmc_phasepoint* z_out, const ahmc_stats* stats,
@@ -284,7 +292,9 @@ int ahmc_nuts_adapt_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahm
  * chain's dual averaging fed by its transition's acceptance_rate = min(1, exp(H0 - H')).  Same cfg, requirements and
  * errors as ahmc_nuts_adapt_sample_f64 (Diag metric, Philox randomness, 0 <= n_adapts <= n_transitions); partial momentum
  * refreshment and tempering as in ahmc_hmc_sample_f64.  n_adapts = 0 gives ahmc_hmc_sample_f64's results bit for bit.
- * (`FixedIntegrationTime` has no in-launch form: with a per-chain eps its number of steps differs per chain.) */
+ * (`FixedIntegrationTime` has no in-launch form: with a per-chain eps its number of steps differs per chain.)
+ * D > 512: streamed, without tempering; the chain's M^-1 is read from its Minv_chain row (required with adapt_metric),
+ * and the estimator state takes 2 (WelfordVar) or 4 (NutpieVar) more workspace D-vectors per chain. */
 int ahmc_hmc_adapt_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, int32_t D, int64_t N,
                               int32_t n_steps, int32_t n_transitions, const ahmc_adapt_cfg* cfg, const ahmc_rng* rng,
                               const ahmc_phasepoint* z_in, const ahmc_phasepoint* z_out, double* draws,
@@ -293,7 +303,9 @@ int ahmc_hmc_adapt_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc
 /* `find_good_stepsize(rng, h, theta)` (src/trajectory.jl:768-837) for N chains at once, each running its own search, in
  * ONE launch: momentum draw (rng->normal_tape or Philox), the direction probe, the crossing loop and the bisection, every
  * probe `A(h, z, eps)` (:753-757) one leapfrog step.  z: theta + the cached lp_value / lp_gradient (ahmc_phasepoint_f64);
- * eps_out[N]; r_out (nullable, D x N with z->ld) receives the momenta used.  No host round trip. */
+ * eps_out[N]; r_out (nullable, D x N with z->ld) receives the momenta used.  No host round trip.  D > 512: every probe is
+ * one streamed `step` from the start point (workspace: 4 D-vectors per chain), so chain c's eps equals the single-chain
+ * search through ahmc_leapfrog_f64 with the same momentum bit for bit. */
 int ahmc_find_good_stepsize_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, int32_t D, int64_t N,
                                 const ahmc_phasepoint* z, const ahmc_rng* rng, double initial_step_size, int32_t max_n_iters,
                                 double* eps_out, double* r_out, uint32_t flags);
