@@ -46,7 +46,7 @@ class AdaptCfg(C.Structure):
     _fields_ = [("n_adapts", C.c_int32), ("init_buffer", C.c_int32), ("term_buffer", C.c_int32), ("window_size", C.c_int32),
                 ("delta", C.c_double), ("gamma", C.c_double), ("t0", C.c_double), ("kappa", C.c_double),
                 ("adapt_metric", C.c_int32), ("n_min", C.c_int32), ("eps_chain", _vp), ("Minv_chain", _vp),
-                ("eps_trace", _vp)]
+                ("eps_trace", _vp), ("cholU_chain", _vp)]
 
 
 class PooledCfg(C.Structure):

@@ -317,13 +317,34 @@ class DiagEuclideanMetric(AbstractMetric):
 
 
 class DenseEuclideanMetric(AbstractMetric):
-    """src/metric.jl:89-120.  Minv: (D, D); cholU = cholesky(Symmetric(Minv)).U (host LAPACK via numpy)."""
+    """src/metric.jl:89-120.  Minv: (D, D); cholU = cholesky(Symmetric(Minv)).U (host LAPACK via numpy).
+
+    Minv: (N, D, D) is a per-chain M^-1 (the reference's `AbstractArray{T,3}` form, metric.jl:89-103; D <= 512), chain c's
+    matrix Minv[c].  Its upper factors cholU (N, D, D) are computed by a batched Cholesky on the array's own device (numpy on
+    the host, torch.linalg on a GPU tensor) unless they are handed in -- e.g. the factors an in-launch WelfordCov warm-up
+    returns, so that sampling continues without refactorising.  Like `cholesky(Symmetric(M^-1)).U` and the launch's own
+    factorisation they read the upper triangle (an adapted M^-1 is not symmetrised)."""
 
     kind = L.METRIC_DENSE
 
-    def __init__(self, Minv):
+    def __init__(self, Minv, cholU=None):
         if isinstance(Minv, int):
             Minv = np.eye(Minv)
+        self.per_chain = Minv.ndim == 3
+        if self.per_chain:
+            if Minv.shape[1] != Minv.shape[2]:
+                raise L.InvalidArgument(L.ERR_INVALID, f"per-chain Minv must be (N, D, D), got {tuple(Minv.shape)}")
+            if cholU is None:
+                # the lower factor of the transpose reads the upper triangle: U = chol(M^T).L^T
+                if _is_host(Minv):
+                    cholU = np.linalg.cholesky(np.asarray(Minv, dtype=np.float64).transpose(0, 2, 1)).transpose(0, 2, 1)
+                else:
+                    cholU = torch.linalg.cholesky(Minv.to(torch.float64).mT).mT
+            if tuple(cholU.shape) != tuple(Minv.shape):
+                raise L.InvalidArgument(L.ERR_INVALID, f"cholU has shape {tuple(cholU.shape)}, Minv {tuple(Minv.shape)}")
+            self.Minv, self.cholU = Minv, cholU
+            self.size = (Minv.shape[1], Minv.shape[0])
+            return
         Mh = Minv if _is_host(Minv) else Minv.detach().cpu().numpy()
         self.Minv = Minv
         self._Minv_h = np.ascontiguousarray(Mh, dtype=np.float64)
@@ -331,6 +352,13 @@ class DenseEuclideanMetric(AbstractMetric):
         self.size = (Mh.shape[0],)
 
     def _desc(self, D, N, like):
+        if self.per_chain:
+            if tuple(self.Minv.shape) != (N, D, D):
+                raise L.InvalidArgument(L.ERR_INVALID, f"AxesMismatch: per-chain Minv is {tuple(self.Minv.shape)} but r is ({N},{D})")
+            # chain c's column-major D x D matrices at D*D*c: each chain's matrix transposed, row-major
+            Mi = _coerce_like(self.Minv.transpose(0, 2, 1) if _is_host(self.Minv) else self.Minv.mT, like)
+            U = _coerce_like(self.cholU.transpose(0, 2, 1) if _is_host(self.cholU) else self.cholU.mT, like)
+            return L.Metric(L.METRIC_DENSE, _ptr(Mi), D * D, _ptr(U)), (Mi, U)
         if self._Minv_h.shape != (D, D):
             raise L.InvalidArgument(L.ERR_INVALID, f"AxesMismatch: Minv is {self._Minv_h.shape} but r has {D} rows")
         # column-major D x D == transposed row-major; Minv symmetric, U stored column-major
@@ -993,7 +1021,9 @@ class VectorisedStanAdaptor:
     adaptors -- one dual-averaging state and one windowed variance estimator PER CHAIN (stepsize.jl:178-210,
     massmatrix.jl:141-157, stan_adaptor.jl:13-50, 137-159).  Runs inside the NUTS launch (ahmc_nuts_adapt_sample_f64)
     or the static-HMC launch (ahmc_hmc_adapt_sample_f64).  metric_estimator: "welford" (`WelfordVar((D, N))` of the
-    positions) or "nutpie" (`NutpieVar((D, N))`, massmatrix.jl:172-250: positions and gradients)."""
+    positions), "nutpie" (`NutpieVar((D, N))`, massmatrix.jl:172-250: positions and gradients) or, with a
+    DenseEuclideanMetric (shared or per chain), "welford_cov" (one `WelfordCov(D)` per chain, massmatrix.jl:284-340).  A
+    Dense metric with adapt_metric = False adapts the step size only."""
     delta: float = 0.8
     adapt_metric: bool = True
     init_buffer: int = 75
@@ -1006,7 +1036,9 @@ class VectorisedStanAdaptor:
     metric_estimator: str = "welford"
 
 
-_ESTIMATORS = {"welford": 1, "nutpie": 2}  # ahmc_adapt_cfg.adapt_metric (AHMC_ADAPT_WELFORD / AHMC_ADAPT_NUTPIE)
+# ahmc_adapt_cfg.adapt_metric (AHMC_ADAPT_WELFORD / AHMC_ADAPT_NUTPIE / AHMC_ADAPT_WELFORD_COV)
+_ESTIMATORS = {"welford": 1, "nutpie": 2, "welford_cov": 3}
+_WELFORD_COV = 3
 
 
 def _adapt_launch_args(h: Hamiltonian, kappa: HMCKernel, z: PhasePoint, n_transitions: int, n_adapts: int,
@@ -1026,11 +1058,20 @@ def _adapt_launch_args(h: Hamiltonian, kappa: HMCKernel, z: PhasePoint, n_transi
         eps[...] = np.asarray(e0, dtype=np.float64)
     else:
         eps.copy_(e0 if hasattr(e0, "detach") else torch.as_tensor(np.asarray(e0, dtype=np.float64)))
-    minv = _like(z.theta, (N, D)) if adaptor.adapt_metric else None
+    est = _ESTIMATORS[adaptor.metric_estimator] if adaptor.adapt_metric else 0
+    cov = est == _WELFORD_COV
+    if cov and not isinstance(h.metric, DenseEuclideanMetric):
+        raise L.InvalidArgument(L.ERR_INVALID, "metric_estimator='welford_cov' adapts a dense M^-1: it needs a DenseEuclideanMetric")
+    # WelfordCov: the chains' M^-1 and factors, column-major D x D per chain (each chain's matrix transposed, row-major)
+    minv = _like(z.theta, (N, D, D) if cov else (N, D)) if adaptor.adapt_metric else None
+    cholu = _like(z.theta, (N, D, D)) if cov else None
     trace = _like(z.theta, (n_transitions, N)) if keep_eps_trace else None
     cfg = L.AdaptCfg(n_adapts, adaptor.init_buffer, adaptor.term_buffer, adaptor.window_size, adaptor.delta, adaptor.gamma,
-                     adaptor.t0, adaptor.kappa, _ESTIMATORS[adaptor.metric_estimator] if adaptor.adapt_metric else 0,
-                     adaptor.n_min, _ptr(eps), _ptr(minv), _ptr(trace))
+                     adaptor.t0, adaptor.kappa, est, adaptor.n_min, _ptr(eps), _ptr(minv), _ptr(trace), _ptr(cholu))
+    if cov:  # the adapted metric as a per-chain DenseEuclideanMetric: its factors come from the launch, not a refactorisation
+        tr = (lambda a: a.transpose(0, 2, 1)) if host else (lambda a: a.mT)
+        keep = keep + (minv, cholu)
+        minv = DenseEuclideanMetric(tr(minv), cholU=tr(cholu))
     rc = L.Rng(rng.seed, rng.offset, None, None, 0, None, 0, _refresh_alpha(kappa), _temper_alpha(kappa.tau.integrator))
     draws = _like(z.theta, (n_transitions, N, D)) if keep_draws else None
     return N, D, host, out, md, keep, eps, minv, trace, cfg, rc, draws
@@ -1039,9 +1080,13 @@ def _adapt_launch_args(h: Hamiltonian, kappa: HMCKernel, z: PhasePoint, n_transi
 def nuts_adapt_sample(rng: PhiloxRNG, h: Hamiltonian, kappa: HMCKernel, z: PhasePoint, n_transitions: int, n_adapts: int,
                       adaptor: VectorisedStanAdaptor, keep_draws: bool = True, keep_eps_trace: bool = False, flags: int = 0):
     """n_adapts adapting + (n_transitions - n_adapts) sampling NUTS transitions per chain in ONE launch, every chain
-    adapting its own step size (and diagonal metric).  -> (z_last, draws (T, N, D) | None, stats of (T, N) arrays,
+    adapting its own step size (and metric).  -> (z_last, draws (T, N, D) | None, stats of (T, N) arrays,
     eps (N,), Minv (N, D) | None, eps_trace (T, N) | None).  The initial step size is `step_size(kappa.tau.integrator)`
-    (scalar or per chain), the initial metric h.metric (DiagEuclideanMetric)."""
+    (scalar or per chain), the initial metric h.metric (DiagEuclideanMetric, or DenseEuclideanMetric shared or per chain).
+    With metric_estimator="welford_cov" the Minv slot is a per-chain DenseEuclideanMetric: its .Minv holds the (N, D, D)
+    adapted M^-1 and its .cholU the (N, D, D) upper factors the launch computed.  To continue sampling with the result,
+    build Hamiltonian(that metric, h.target) and call sample_transitions(rng, h2, kappa with Leapfrog(eps), z_last, n):
+    no refactorisation happens.  Chain c's M^-1 is replaced only at window ends whose Cholesky factorisation succeeds."""
     if not isinstance(rng, PhiloxRNG):
         raise L.InvalidArgument(L.ERR_INVALID, "in-launch adaptation draws from the on-device Philox streams")
     tau = kappa.tau
@@ -1067,7 +1112,9 @@ def hmc_adapt_sample(rng: PhiloxRNG, h: Hamiltonian, kappa: HMCKernel, z: PhaseP
     """`nuts_adapt_sample` for static HMC (`Trajectory{EndPointTS}(Leapfrog | TemperedLeapfrog, FixedNSteps(n))`): n_adapts
     adapting + (n_transitions - n_adapts) sampling transitions per chain in ONE launch (ahmc_hmc_adapt_sample_f64), each
     chain's dual averaging fed by its own acceptance rate min(1, exp(H0 - H')).  Same return tuple:
-    (z_last, draws | None, stats of (T, N) arrays, eps (N,), Minv (N, D) | None, eps_trace (T, N) | None)."""
+    (z_last, draws | None, stats of (T, N) arrays, eps (N,), Minv (N, D) | None, eps_trace (T, N) | None); with
+    metric_estimator="welford_cov" the Minv slot is the per-chain DenseEuclideanMetric of the adapted M^-1 and factors
+    (see nuts_adapt_sample for continuing with it)."""
     if not isinstance(rng, PhiloxRNG):
         raise L.InvalidArgument(L.ERR_INVALID, "in-launch adaptation draws from the on-device Philox streams")
     tau = kappa.tau

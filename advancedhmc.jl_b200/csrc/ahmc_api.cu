@@ -217,6 +217,9 @@ int check_common(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metr
         if (metric->kind == AHMC_METRIC_DIAG && metric->chain_stride != 0 && metric->chain_stride < D)
             return fail(ctx, AHMC_ERR_INVALID, "AxesMismatch: per-chain Minv stride %lld < D=%d (hamiltonian.jl:53-57)",
                         (long long)metric->chain_stride, D);
+        if (metric->kind == AHMC_METRIC_DENSE && metric->chain_stride != 0 && metric->chain_stride < (int64_t)D * D)
+            return fail(ctx, AHMC_ERR_INVALID, "AxesMismatch: per-chain dense Minv / cholU stride %lld < D*D=%lld (metric.jl:89-103)",
+                        (long long)metric->chain_stride, (long long)D * D);
     }
     int G, E;
     if (!pick_layout(D, &G, &E)) {
@@ -255,25 +258,28 @@ int check_pp(ahmc_ctx* ctx, const ahmc_phasepoint* z, int32_t D, const char* nam
 
 size_t metric_minv_count(const ahmc_metric* m, int32_t D, int64_t N) {
     if (m->kind == AHMC_METRIC_DIAG) return m->chain_stride ? (size_t)m->chain_stride * (size_t)N : (size_t)D;
-    if (m->kind == AHMC_METRIC_DENSE) return (size_t)D * D;
+    if (m->kind == AHMC_METRIC_DENSE)  // per chain: chain c's matrix at chain_stride * c (the last one D*D long)
+        return m->chain_stride && N > 0 ? (size_t)m->chain_stride * (size_t)(N - 1) + (size_t)D * D : (size_t)D * D;
     return 0;
 }
+bool per_chain_dense(const ahmc_metric* m) { return m->kind == AHMC_METRIC_DENSE && m->chain_stride != 0; }
 
 ModelDev model_dev(const ahmc_model* m) { return ModelDev{m->kind, m->D, m->d_p0, m->d_p1, m->c0, m->rtc, m->d_p1_coop}; }
 
 // stage the metric descriptor (device or host pointers) into a MetricDev
 int stage_metric(Stager& st, const ahmc_metric* m, int32_t D, int64_t N, MetricDev* out) {
     out->kind = m->kind;
-    out->chain_stride = m->kind == AHMC_METRIC_DIAG ? m->chain_stride : 0;
+    out->chain_stride = m->kind != AHMC_METRIC_UNIT ? m->chain_stride : 0;
     out->Minv_coop = nullptr;
     out->cholU_coop = nullptr;
     int rc = st.in(m->Minv, metric_minv_count(m, D, N), &out->Minv);
     if (rc) return rc;
-    return st.in(m->kind == AHMC_METRIC_DENSE ? m->cholU : (const double*)nullptr, (size_t)D * D, &out->cholU);
+    // a Dense factor has the layout of its M^-1 (shared, or per chain at the same stride)
+    return st.in(m->kind == AHMC_METRIC_DENSE ? m->cholU : (const double*)nullptr, metric_minv_count(m, D, N), &out->cholU);
 }
 void reserve_metric(Stager& st, const ahmc_metric* m, int32_t D, int64_t N) {
     st.reserve(metric_minv_count(m, D, N) * sizeof(double));
-    if (m->kind == AHMC_METRIC_DENSE) st.reserve((size_t)D * D * sizeof(double));
+    if (m->kind == AHMC_METRIC_DENSE) st.reserve(metric_minv_count(m, D, N) * sizeof(double));
 }
 
 int finish_call(ahmc_ctx* ctx, Stager& st, uint32_t flags) {
@@ -374,7 +380,7 @@ int try_dense_trajectory(ahmc_ctx* ctx, const ahmc_model* model, LeapfrogArgs& a
     const long long N = a.N;
     const bool gauss = model->kind == AHMC_MODEL_STD_NORMAL || model->kind == AHMC_MODEL_DIAG_GAUSS ||
                        model->kind == AHMC_MODEL_DENSE_GAUSS;
-    const bool metric_ok = a.metric.kind != AHMC_METRIC_DIAG || a.metric.chain_stride == 0;
+    const bool metric_ok = a.metric.chain_stride == 0;  // the tile kernel shares one M^-1 across its chains
     const bool has_dense = model->kind == AHMC_MODEL_DENSE_GAUSS || a.metric.kind == AHMC_METRIC_DENSE;
     int Dp, RB, CB;
     if (!(gauss && metric_ok && has_dense && !compat && a.g_in && !(a.flags & AHMC_FLAG_EXACT_CHECKS) && !(temper_alpha > 0.0) &&
@@ -1220,30 +1226,65 @@ static int stage_rng(Stager& st, const ahmc_rng* r, int32_t D, int64_t N, bool n
 
 // ---- in-launch adaptation (ahmc_nuts_adapt_sample_f64, ahmc_hmc_adapt_sample_f64): the cfg checks after the metric /
 // sampler family checks of each entry point, the staging of the adaptors' buffers, and the per-chain workspace
+// The metric / estimator pairs an adaptive launch accepts, checked before everything else of the cfg: the diagonal
+// estimators adapt a Diag metric; a Dense metric (shared or per chain, as the starting point) adapts its step size only or
+// runs WelfordCov, on built-in targets.
+static int check_adapt_metric(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, const ahmc_adapt_cfg* cfg) {
+    if (cfg->adapt_metric == AHMC_ADAPT_WELFORD_COV && metric->kind != AHMC_METRIC_DENSE)
+        return fail(ctx, AHMC_ERR_INVALID, "cfg.adapt_metric = AHMC_ADAPT_WELFORD_COV adapts a dense M^-1: it needs the Dense metric");
+    if (metric->kind == AHMC_METRIC_DENSE) {
+        if (cfg->adapt_metric != AHMC_ADAPT_STEPSIZE && cfg->adapt_metric != AHMC_ADAPT_WELFORD_COV)
+            return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation of a Dense metric: AHMC_ADAPT_STEPSIZE or AHMC_ADAPT_WELFORD_COV "
+                                                   "(WelfordVar / NutpieVar estimate a diagonal M^-1)");
+        if (model->kind == AHMC_MODEL_USER)
+            return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation with a Dense metric is built for the built-in targets; "
+                                                   "run-time compiled targets adapt a Diag metric");
+        // the launch copies the starting factor into the chain's cholU_chain row (and reads the chain's row for every
+        // momentum refresh), so it is required even with AHMC_FLAG_NO_REFRESH
+        if (!metric->cholU)
+            return fail(ctx, AHMC_ERR_INVALID, "in-launch adaptation with a Dense metric needs its cholU (metric.jl:104-109)");
+        return AHMC_OK;
+    }
+    if (metric->kind != AHMC_METRIC_DIAG)
+        return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation needs the Diag metric (per-chain diagonal M^-1) or the Dense metric");
+    return AHMC_OK;
+}
 static int check_adapt_cfg(ahmc_ctx* ctx, const ahmc_adapt_cfg* cfg, const ahmc_rng* rng, int32_t n_transitions) {
     if (rng->normal_tape || rng->exp_tape || rng->dir_tape)
         return fail(ctx, AHMC_ERR_INVALID, "in-launch adaptation draws from the Philox streams (no tapes)");
     if (cfg->n_adapts < 0 || cfg->n_adapts > n_transitions)
         return fail(ctx, AHMC_ERR_INVALID, "need 0 <= n_adapts <= n_transitions");
     if (!cfg->eps_chain) return fail(ctx, AHMC_ERR_INVALID, "cfg.eps_chain (N, in/out) is required");
-    if (cfg->adapt_metric < AHMC_ADAPT_STEPSIZE || cfg->adapt_metric > AHMC_ADAPT_NUTPIE)
-        return fail(ctx, AHMC_ERR_INVALID, "cfg.adapt_metric must be AHMC_ADAPT_STEPSIZE (0), AHMC_ADAPT_WELFORD (1) or AHMC_ADAPT_NUTPIE (2)");
+    if (cfg->adapt_metric < AHMC_ADAPT_STEPSIZE || cfg->adapt_metric > AHMC_ADAPT_WELFORD_COV)
+        return fail(ctx, AHMC_ERR_INVALID, "cfg.adapt_metric must be AHMC_ADAPT_STEPSIZE (0), AHMC_ADAPT_WELFORD (1), AHMC_ADAPT_NUTPIE (2) "
+                                           "or AHMC_ADAPT_WELFORD_COV (3)");
     if (cfg->adapt_metric && !cfg->Minv_chain)
-        return fail(ctx, AHMC_ERR_INVALID, "cfg.Minv_chain (N x D, out) is required with adapt_metric");
+        return fail(ctx, AHMC_ERR_INVALID, "cfg.Minv_chain (N x D, out; N x D x D with WelfordCov) is required with adapt_metric");
+    if (cfg->adapt_metric == AHMC_ADAPT_WELFORD_COV && !cfg->cholU_chain)
+        return fail(ctx, AHMC_ERR_INVALID, "cfg.cholU_chain (N x D x D, out) is required with AHMC_ADAPT_WELFORD_COV");
     if (cfg->init_buffer < 0 || cfg->term_buffer < 0 || cfg->window_size < 1)
         return fail(ctx, AHMC_ERR_INVALID, "need init_buffer >= 0, term_buffer >= 0, window_size >= 1");
     if (!(cfg->gamma > 0.0) || !(cfg->t0 >= 0.0) || !(cfg->delta > 0.0 && cfg->delta < 1.0))
         return fail(ctx, AHMC_ERR_INVALID, "need gamma > 0, t0 >= 0, 0 < delta < 1");
     return AHMC_OK;
 }
-static void reserve_adapt(Stager& st, const ahmc_adapt_cfg* cfg, int32_t D, int64_t N, int32_t n_transitions) {
+// doubles of one chain's Minv_chain row: D, or D x D for a Dense metric (its rows also need the cholU_chain row; with step
+// size only both are optional and, when given, receive the starting metric)
+static size_t adapt_row_doubles(const ahmc_metric* metric, int32_t D) {
+    return metric->kind == AHMC_METRIC_DENSE ? (size_t)D * D : (size_t)D;
+}
+static bool dense_rows(const ahmc_metric* metric, const ahmc_adapt_cfg* cfg) {
+    return metric->kind == AHMC_METRIC_DENSE && cfg->Minv_chain && cfg->cholU_chain;
+}
+static void reserve_adapt(Stager& st, const ahmc_metric* metric, const ahmc_adapt_cfg* cfg, int32_t D, int64_t N, int32_t n_transitions) {
     st.reserve((size_t)N * 8);
-    if (cfg->Minv_chain) st.reserve((size_t)N * D * 8);
+    if (cfg->Minv_chain) st.reserve((size_t)N * adapt_row_doubles(metric, D) * 8);
+    if (dense_rows(metric, cfg)) st.reserve((size_t)N * D * D * 8);
     if (cfg->eps_trace) st.reserve((size_t)N * n_transitions * 8);
 }
 // fills `ad` (schedule, constants, staged eps / M^-1 / trace buffers); *eps_chain = the per-chain step sizes the kernel reads
-static int stage_adapt(ahmc_ctx* ctx, Stager& st, const ahmc_adapt_cfg* cfg, int32_t D, int64_t N, int32_t n_transitions,
-                       AdaptDev* ad, const double** eps_chain) {
+static int stage_adapt(ahmc_ctx* ctx, Stager& st, const ahmc_metric* metric, const ahmc_adapt_cfg* cfg, int32_t D, int64_t N,
+                       int32_t n_transitions, AdaptDev* ad, const double** eps_chain) {
     ad->enabled = 1;
     ad->n_adapts = cfg->n_adapts;
     ad->delta = cfg->delta;
@@ -1258,7 +1299,16 @@ static int stage_adapt(ahmc_ctx* ctx, Stager& st, const ahmc_adapt_cfg* cfg, int
     int rc;
     if ((rc = st.inout(cfg->eps_chain, (size_t)N, &ad->eps))) return rc;
     *eps_chain = ad->eps;
-    if ((rc = st.out(cfg->Minv_chain, (size_t)N * D, &ad->minv))) return rc;
+    if (metric->kind == AHMC_METRIC_DENSE) {  // the chain's M^-1 / factor rows: both or neither (step size only)
+        ad->minv = ad->cholU = nullptr;
+        if (dense_rows(metric, cfg)) {
+            if ((rc = st.out(cfg->Minv_chain, (size_t)N * D * D, &ad->minv))) return rc;
+            if ((rc = st.out(cfg->cholU_chain, (size_t)N * D * D, &ad->cholU))) return rc;
+        }
+    } else {
+        ad->cholU = nullptr;
+        if ((rc = st.out(cfg->Minv_chain, (size_t)N * D, &ad->minv))) return rc;
+    }
     if ((rc = st.out(cfg->eps_trace, (size_t)N * n_transitions, &ad->eps_trace))) return rc;
     return AHMC_OK;
 }
@@ -1284,11 +1334,11 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
     if (!ctx || !model || !metric || !rng) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/model/metric/rng");
     if (n_transitions < 1) return fail(ctx, AHMC_ERR_INVALID, "n_transitions must be >= 1");
     if (cfg) {
-        if (metric->kind != AHMC_METRIC_DIAG)
-            return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation needs the Diag metric (per-chain diagonal M^-1)");
+        int rc = check_adapt_metric(ctx, model, metric, cfg);
+        if (rc) return rc;
         if (model->kind == AHMC_MODEL_CALLBACK)
             return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation needs a device-resident target: callback (split-step) models cannot run inside one launch; express the target as CUDA source (ahmc_model_create_user)");
-        int rc = check_adapt_cfg(ctx, cfg, rng, n_transitions);
+        rc = check_adapt_cfg(ctx, cfg, rng, n_transitions);
         if (rc) return rc;
     }
     if (n_transitions > 1 && (rng->normal_tape || rng->exp_tape))
@@ -1324,7 +1374,7 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
     st.reserve((size_t)D * N * 8);
     st.reserve((size_t)N * 8 * 16 * n_transitions);
     if (draws) st.reserve((size_t)D * N * n_transitions * 8);
-    if (cfg) reserve_adapt(st, cfg, D, N, n_transitions);
+    if (cfg) reserve_adapt(st, metric, cfg, D, N, n_transitions);
     if ((rc = st.prepare())) return rc;
     HmcArgs h{};
     LeapfrogArgs& a = h.lf;
@@ -1334,7 +1384,7 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
     a.N = N;
     a.eps = eps;
     if (cfg) {
-        if ((rc = stage_adapt(ctx, st, cfg, D, N, n_transitions, &h.ad, &a.eps_chain))) return rc;
+        if ((rc = stage_adapt(ctx, st, metric, cfg, D, N, n_transitions, &h.ad, &a.eps_chain))) return rc;
     } else if ((rc = st.in(eps_chain, (size_t)N, &a.eps_chain))) {
         return rc;
     }
@@ -1410,7 +1460,7 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
         t.th_in = a.th_out; t.r_in = a.r_out; t.g_in = a.g_out; t.ld_in = a.ld_out;
         t.status = nullptr; t.steps_done = nullptr; t.only_mask = nullptr; t.min_break = nullptr;
         const bool gauss = model->kind != AHMC_MODEL_FUNNEL && model->kind != AHMC_MODEL_CALLBACK && model->kind != AHMC_MODEL_USER;
-        const bool metric_ok = a.metric.kind != AHMC_METRIC_DIAG || a.metric.chain_stride == 0;
+        const bool metric_ok = a.metric.chain_stride == 0;  // shared M^-1 (the tile kernel's chains share one matrix)
         int Dp_, RB_, CB_;
         if (gauss && metric_ok && !(flags & AHMC_FLAG_EXACT_CHECKS) && dense_tile_shape(D, &Dp_, &RB_, &CB_)) {
             if (h.refresh) {
@@ -1448,9 +1498,9 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
             }
         }
     }
-    if (cfg || D > 512) {  // the adaptors' estimator state: chain_adapt_vectors D-vectors per chain; at D > 512 also the
+    if (cfg || D > 512) {  // the adaptors' estimator state: chain_adapt_doubles per chain; at D > 512 also the
                            // transition's start point, kBigHmcVectors D-vectors per chain ahead of it (ahmc_bigd_hmc.cu)
-        h.scratch_stride = (long long)((D > 512 ? kBigHmcVectors : 0) + (cfg ? chain_adapt_vectors(cfg->adapt_metric) : 0)) * D;
+        h.scratch_stride = (long long)(D > 512 ? kBigHmcVectors : 0) * D + (cfg ? chain_adapt_doubles(cfg->adapt_metric, D) : 0);
         if ((rc = chain_workspace(ctx, (size_t)h.scratch_stride * (size_t)N * sizeof(double), &h.scratch))) return rc;
     }
     CU(launch_hmc(h, ctx->stream, &nl));
@@ -1465,11 +1515,11 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
     if (!ctx || !model || !metric || !rng) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/model/metric/rng");
     if (n_transitions < 1) return fail(ctx, AHMC_ERR_INVALID, "n_transitions must be >= 1");
     if (cfg) {
-        if (metric->kind != AHMC_METRIC_DIAG)
-            return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation needs the Diag metric (per-chain diagonal M^-1)");
+        int rc = check_adapt_metric(ctx, model, metric, cfg);
+        if (rc) return rc;
         if (flags & (AHMC_FLAG_NUTS_SLICE_TS | AHMC_FLAG_NUTS_CLASSIC | AHMC_FLAG_NUTS_STRICT))
             return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation is built for MultinomialTS + GeneralisedNoUTurn");
-        int rc = check_adapt_cfg(ctx, cfg, rng, n_transitions);
+        rc = check_adapt_cfg(ctx, cfg, rng, n_transitions);
         if (rc) return rc;
     }
     if (n_transitions > 1 && (rng->normal_tape || rng->exp_tape || rng->dir_tape))
@@ -1509,15 +1559,16 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
     if (draws) st.reserve((size_t)D * N * n_transitions * 8);
     if (rng->exp_tape) st.reserve((size_t)rng->exp_stride * N * 8);
     if (rng->dir_tape) st.reserve((size_t)rng->dir_stride * N);
-    if (cfg) reserve_adapt(st, cfg, D, N, n_transitions);
+    if (cfg) reserve_adapt(st, metric, cfg, D, N, n_transitions);
     if ((rc = st.prepare())) return rc;
     NutsArgs a{};
     a.model = model_dev(model);
     if ((rc = stage_metric(st, metric, D, N, &a.metric))) return rc;
     int n_prep = 0;
-    if (a.metric.kind == AHMC_METRIC_DENSE && D > 16 && D <= 512) {
+    if (a.metric.kind == AHMC_METRIC_DENSE && a.metric.chain_stride == 0 && !cfg && D > 16 && D <= 512) {
         // the cooperative form streams Minv / cholU in chunks of columns: hand it copies whose columns are padded to the
-        // shared-memory leading dimension, so that a chunk is one bulk copy (two small kernels per call, on the stream)
+        // shared-memory leading dimension, so that a chunk is one bulk copy (two small kernels per call, on the stream).
+        // (A per-chain Dense metric, and the Dense adaptive form, run warp per chain: no shared matrix to pad.)
         const size_t per = coop_padded_doubles(D);
         if (2 * per > ctx->coop_scratch_doubles) {
             CU(cudaStreamSynchronize(ctx->stream));
@@ -1542,7 +1593,7 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
     a.N = N;
     a.eps = eps;
     if (cfg) {
-        if ((rc = stage_adapt(ctx, st, cfg, D, N, n_transitions, &a.ad, &a.eps_chain))) return rc;
+        if ((rc = stage_adapt(ctx, st, metric, cfg, D, N, n_transitions, &a.ad, &a.eps_chain))) return rc;
     } else if ((rc = st.in(eps_chain, (size_t)N, &a.eps_chain))) {
         return rc;
     }
@@ -1568,7 +1619,7 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
     if ((rc = st.out(draws, (size_t)D * N * n_transitions, &a.draws))) return rc;
     a.n_transitions = n_transitions;
     // per-chain tree workspace
-    a.scratch_stride = nuts_scratch_doubles_per_chain(D, max_depth, cfg ? chain_adapt_vectors(cfg->adapt_metric) : 0);
+    a.scratch_stride = nuts_scratch_doubles_per_chain(D, max_depth, cfg ? chain_adapt_doubles(cfg->adapt_metric, D) : 0);
     if ((rc = chain_workspace(ctx, (size_t)a.scratch_stride * (size_t)N * sizeof(double), &a.scratch))) return rc;
     int nl = 0;
     CU(launch_nuts(a, ctx->stream, &nl));

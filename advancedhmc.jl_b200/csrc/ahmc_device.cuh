@@ -62,6 +62,13 @@ struct ModelDev {
 template <int MODEL>
 __host__ __device__ constexpr int slab_vectors() { return MODEL == AHMC_MODEL_USER ? 2 : 1; }
 
+// The template metric kind of a per-chain Dense metric (chain_stride >= D*D: chain c's M^-1 and factor at chain_stride*c),
+// internal to the kernels -- the C ABI's kind stays AHMC_METRIC_DENSE.  Its kernels are instantiations of their own, so the
+// shared-matrix Dense kernels are compiled exactly as before: only these index the matrices by the chain, and they read
+// them with coherent loads, because the in-launch WelfordCov warm-up writes a chain's rows during the launch.
+constexpr int kMetricDenseChain = 3;
+__host__ __device__ constexpr bool is_dense_metric(int kind) { return kind == AHMC_METRIC_DENSE || kind == kMetricDenseChain; }
+
 struct MetricDev {
     int kind;
     const double* Minv;
@@ -70,6 +77,10 @@ struct MetricDev {
     const double* Minv_coop;   // Dense, nullable: Minv / cholU with padded columns (see ModelDev::p1_coop)
     const double* cholU_coop;
 };
+// the template metric kind a launch instantiates for this metric: kMetricDenseChain for a per-chain Dense metric
+__host__ __device__ inline int metric_form(const MetricDev& m) {
+    return m.kind == AHMC_METRIC_DENSE && m.chain_stride != 0 ? kMetricDenseChain : m.kind;
+}
 
 // ------------------------------------------------------------------------------------------------
 // group collectives
@@ -470,6 +481,28 @@ __device__ __forceinline__ void matvec_coop(const double* __restrict__ A, const 
     }
 }
 
+// matvec for a chain's own matrix (kMetricDenseChain), which the same launch may write: coherent loads, no read-only path
+template <int G, int E>
+__device__ __forceinline__ void matvec_coherent(const double* A, int D, const double (&x)[E], double (&y)[E], double* xs, int l) {
+    __syncwarp();
+#pragma unroll
+    for (int e = 0; e < E; ++e) {
+        int d = l + G * e;
+        if (d < D) xs[d] = x[e];
+        y[e] = 0.0;
+    }
+    __syncwarp();
+    for (int k = 0; k < D; ++k) {
+        double xk = xs[k];
+        const double* col = A + (long long)D * k;
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            int d = l + G * e;
+            if (d < D) y[e] = fma(col[d], xk, y[e]);
+        }
+    }
+}
+
 // solve U x = z (U upper triangular, column-major) for a group-distributed vector; result in x.
 // Back substitution, one pivot per iteration (metric.jl:311-320 `ldiv!(cholMinv, r)`).
 template <int G, int E>
@@ -489,6 +522,28 @@ __device__ __forceinline__ void upper_solve(const double* __restrict__ U, int D,
                 x[e] = xi;
             else if (d < i)
                 x[e] = fma(-__ldg(col + d), xi, x[e]);
+        }
+    }
+}
+
+// upper_solve for a chain's own factor (kMetricDenseChain): coherent loads, as matvec_coherent
+template <int G, int E>
+__device__ __forceinline__ void upper_solve_coherent(const double* U, int D, double (&x)[E], int l) {
+    for (int i = D - 1; i >= 0; --i) {
+        int le = i % G, ee = i / G;
+        double xi = 0.0;
+#pragma unroll
+        for (int e = 0; e < E; ++e)
+            if (e == ee) xi = x[e];
+        xi = Grp<G>::bcast(xi, le) / U[i + (long long)D * i];
+        const double* col = U + (long long)D * i;
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            int d = l + G * e;
+            if (d == i)
+                x[e] = xi;
+            else if (d < i)
+                x[e] = fma(-col[d], xi, x[e]);
         }
     }
 }
@@ -594,10 +649,11 @@ __device__ __forceinline__ void upper_solve_coop(const double* __restrict__ U, c
 // ------------------------------------------------------------------------------------------------
 // metric:  dH/dr and the kinetic lane-partial  sum_e r_e * (dH/dr)_e   (neg_energy = -sum/2)
 // ------------------------------------------------------------------------------------------------
+// METRIC: AHMC_METRIC_UNIT / _DIAG / _DENSE (one shared matrix), or kMetricDenseChain (chain c's own matrices)
 template <int METRIC, int G, int E>
 struct MetricOps {
     double Minv[E];  // Diag only
-    const double* A; // Dense only
+    const double* A; // Dense only: M^-1 (kMetricDenseChain: the chain's own)
     const double* U;
     const double *Ac, *Uc;  // their padded copies for the cooperative products (nullable)
     int D;
@@ -612,6 +668,9 @@ struct MetricOps {
         Uc = m.cholU_coop;
         if (METRIC == AHMC_METRIC_DIAG) {
             vload<G, E>(Minv, m.Minv + m.chain_stride * chain, l, D);
+        } else if (METRIC == kMetricDenseChain) {
+            A = m.Minv + m.chain_stride * chain;
+            U = m.cholU ? m.cholU + m.chain_stride * chain : nullptr;
         }
     }
     // dr = dH/dr(r)   (hamiltonian.jl:50-68)
@@ -622,6 +681,8 @@ struct MetricOps {
         } else if (METRIC == AHMC_METRIC_DIAG) {
 #pragma unroll
             for (int e = 0; e < E; ++e) dr[e] = Minv[e] * r[e];
+        } else if (METRIC == kMetricDenseChain) {
+            matvec_coherent<G, E>(A, D, r, dr, xs, l);
         } else {
             if (G == 32 && coop) matvec_coop<E>(A, Ac, D, r, dr, coop, l);
             else matvec<G, E>(A, D, r, dr, xs, l);
@@ -638,6 +699,8 @@ struct MetricOps {
         } else if (METRIC == AHMC_METRIC_DENSE) {
             if (G == 32 && coop) upper_solve_coop<E>(U, Uc, D, r, coop, l);
             else upper_solve<G, E>(U, D, r, l);
+        } else if (METRIC == kMetricDenseChain) {
+            upper_solve_coherent<G, E>(U, D, r, l);
         }
     }
 };

@@ -87,7 +87,7 @@ struct RngDev {
 };
 
 // in-kernel per-chain adaptation (adaptive K2 / K3 forms, ahmc_chain_adapt.cuh): NesterovDualAveraging + a windowed
-// WelfordVar or NutpieVar per chain
+// WelfordVar, NutpieVar or (Dense metric) WelfordCov per chain
 struct AdaptDev {
     int enabled;
     int n_adapts;                  // iterations 1..n_adapts adapt (sampler.jl:72-90)
@@ -95,11 +95,13 @@ struct AdaptDev {
     int n_splits;
     int splits[12];
     double delta, gamma, t0, kappa;  // stepsize.jl:162-172
-    int adapt_metric;                // AHMC_ADAPT_STEPSIZE / _WELFORD / _NUTPIE
+    int adapt_metric;                // AHMC_ADAPT_STEPSIZE / _WELFORD / _NUTPIE / _WELFORD_COV
     int n_min;                       // massmatrix.jl:103-107
     double* eps;                     // N, out: adapted step size per chain (in: a.eps_chain / a.eps)
-    double* minv;                    // N*D, out: adapted diagonal M^-1 per chain (nullable when !adapt_metric)
+    double* minv;                    // N*D, out: adapted diagonal M^-1 per chain (nullable when !adapt_metric);
+                                     // WelfordCov: N*D*D, the chain's dense M^-1, read and written by the launch
     double* eps_trace;               // nullable, n_transitions x N: step size used by each transition
+    double* cholU;                   // WelfordCov: N*D*D, the upper Cholesky factor of the chain's M^-1 (else nullptr)
 };
 // initialize!(StanHMCAdaptorState, init_buffer, term_buffer, window_size, n_adapts) (stan_adaptor.jl:13-50): the
 // host side of the in-launch adaptation.  false: the schedule needs more window splits than AdaptDev holds.
@@ -123,6 +125,10 @@ inline bool stan_window_schedule(AdaptDev& ad, int init_buffer, int term_buffer,
 // the compiled estimator form (ahmc_chain_adapt.cuh) an adaptive launch needs: NutpieVar has its own, step size only and
 // WelfordVar share one
 inline int adapt_form(const AdaptDev& ad) { return ad.adapt_metric == AHMC_ADAPT_NUTPIE ? AHMC_ADAPT_NUTPIE : AHMC_ADAPT_WELFORD; }
+// the form for a Dense metric (step size only or WelfordCov)
+inline int adapt_form(const AdaptDev& ad, int metric_kind) {
+    return metric_kind == AHMC_METRIC_DENSE ? AHMC_ADAPT_WELFORD_COV : adapt_form(ad);
+}
 
 struct HmcArgs {
     LeapfrogArgs lf;  // th_in/r_in/g_in/lp_in = current phase point; outputs = new phase point
@@ -294,7 +300,7 @@ cudaError_t launch_rand_momentum_big(const MomentumArgs& a, cudaStream_t st);
 cudaError_t launch_hmc_big(const HmcArgs& a, cudaStream_t st);
 cudaError_t launch_find_eps_big(const FindEpsArgs& a, cudaStream_t st);
 cudaError_t launch_nuts(const NutsArgs& a, cudaStream_t stream, int* n_launches);
-long long nuts_scratch_doubles_per_chain(int D, int max_depth, int adapt_vectors);  // + adapt_vectors D-vectors
+long long nuts_scratch_doubles_per_chain(int D, int max_depth, long long adapt_doubles);  // + the estimator state
 cudaError_t launch_trajectory(const TrajArgs& a, cudaStream_t stream, int* n_launches);
 cudaError_t launch_multinomial(const MultinomialArgs& a, cudaStream_t stream, int* n_launches);
 cudaError_t launch_kick_drift(const SplitArgs& a, cudaStream_t stream, int* n_launches);
@@ -345,7 +351,7 @@ constexpr int kBlockThreads = 128;
 
 // dynamic shared memory needed by the dense paths: one D-double slab per group
 inline size_t smem_bytes(int model_kind, int metric_kind, int D, int G) {
-    bool dense = (model_kind == AHMC_MODEL_DENSE_GAUSS) || (metric_kind == AHMC_METRIC_DENSE) || (model_kind == AHMC_MODEL_USER);
+    bool dense = (model_kind == AHMC_MODEL_DENSE_GAUSS) || is_dense_metric(metric_kind) || (model_kind == AHMC_MODEL_USER);
     return dense ? (size_t)(kBlockThreads / G) * (size_t)(model_kind == AHMC_MODEL_USER ? 2 : 1) * (size_t)D * sizeof(double) : 0;
 }
 

@@ -108,11 +108,11 @@ constexpr int min_blocks_per_sm() {
 // alone it takes ~140 and loses a block per SM.
 template <int MODEL, int METRIC, int E>
 constexpr int min_blocks_hmc() {
-    return (FastCapable<MODEL, METRIC>::value && E <= 4) ? 7 : ((METRIC != AHMC_METRIC_DENSE && MODEL != AHMC_MODEL_DENSE_GAUSS && E <= 4) ? 4 : 1);
+    return (FastCapable<MODEL, METRIC>::value && E <= 4) ? 7 : ((!is_dense_metric(METRIC) && MODEL != AHMC_MODEL_DENSE_GAUSS && E <= 4) ? 4 : 1);
 }
 template <int MODEL, int METRIC, int E>
 constexpr int min_blocks_lf() {
-    return (MODEL == AHMC_MODEL_FUNNEL && METRIC != AHMC_METRIC_DENSE && E <= 4) ? 7 : min_blocks_per_sm<MODEL, METRIC, E>();
+    return (MODEL == AHMC_MODEL_FUNNEL && !is_dense_metric(METRIC) && E <= 4) ? 7 : min_blocks_per_sm<MODEL, METRIC, E>();
 }
 
 template <int MODEL, int METRIC, int G, int E, bool CONTIG = false>
@@ -229,15 +229,20 @@ __global__ void __launch_bounds__(kBlockThreads, min_blocks_hmc<MODEL, METRIC, E
     const int D = a.D;
     double* xs = smem + (size_t)grp_in_block * slab_vectors<MODEL>() * D;
     double eps = a.eps_chain ? __ldg(a.eps_chain + chain) : a.eps;
+    constexpr bool kCov = ADAPT == AHMC_ADAPT_WELFORD_COV;  // (METRIC = kMetricDenseChain: the chain's own rows)
 
     MetricOps<METRIC, G, E> me;
-    me.load(a.metric, chain, l, D);
-    HmcIO<METRIC, G, E, (ADAPT != 0)> io{h, chain, l};
-    ChainAdapt<G, E, ADAPT == AHMC_ADAPT_NUTPIE ? AHMC_ADAPT_NUTPIE : AHMC_ADAPT_WELFORD> cad{};
+    MetricDev rows;
+    const MetricDev& md = adapt_launch_metric<ADAPT>(a.metric, h.ad, D, rows);
+    if constexpr (!kCov) me.load(md, chain, l, D);
+    HmcIO<METRIC, G, E, (ADAPT != 0 && !kCov)> io{h, chain, l};
+    ChainAdapt<G, E, ADAPT == AHMC_ADAPT_NUTPIE ? AHMC_ADAPT_NUTPIE : (kCov ? AHMC_ADAPT_WELFORD_COV : AHMC_ADAPT_WELFORD)> cad{};
     if constexpr (ADAPT) {
         __syncwarp();  // every lane has read its starting eps (ad.eps) before lane 0 writes it back
+        if constexpr (kCov) cad.begin_dense(h.ad, a.metric, h.scratch + h.scratch_stride * chain, valid, chain, l, D);
         if (valid) cad.begin(h.ad, h.scratch + h.scratch_stride * chain, eps, me.Minv, chain, l, D);
     }
+    if constexpr (kCov) me.load(md, chain, l, D);  // the rows begin_dense filled
     for (int t = 0; t < h.n_transitions; ++t) {
         const bool first = (t == 0);
         io.src_th = first ? a.th_in + a.ld_in * chain : a.th_out + a.ld_out * chain;
@@ -270,12 +275,15 @@ __global__ void __launch_bounds__(kBlockThreads, min_blocks_hmc<MODEL, METRIC, E
         io.lp0 = map_nonfinite(first ? a.lp_in[chain] : a.lp_out[chain]);
         io.H0 = -(io.lp0 + io.lk0);
         io.ex = h.rng.exp_tape ? h.rng.exp_tape[chain] : philox_exp(h.rng.seed, off, chain, 0);
-        if constexpr (ADAPT) {
+        if constexpr (ADAPT && !kCov) {
 #pragma unroll
             for (int e = 0; e < E; ++e) io.minv[e] = me.Minv[e];
         }
-        run_trajectory<MODEL, METRIC, G, E>(a.model, a.metric, D, chain, valid, l, xs, eps, a.n_steps, h.rng.temper_alpha, a.flags, io);
-        if constexpr (ADAPT) {  // iteration t + 1 of `sample` (sampler.jl:182)
+        run_trajectory<MODEL, METRIC, G, E>(a.model, md, D, chain, valid, l, xs, eps, a.n_steps, h.rng.temper_alpha, a.flags, io);
+        if constexpr (kCov) {  // every lane of the warp calls (the estimator exchanges data across the group)
+            cad.update_cov(h.ad, h.scratch + h.scratch_stride * chain, valid, t + 1, io.stat_idx, io.alpha, a.th_out + a.ld_out * chain,
+                           eps, chain, l, D);
+        } else if constexpr (ADAPT) {  // iteration t + 1 of `sample` (sampler.jl:182)
             if (valid)
                 cad.update(h.ad, h.scratch + h.scratch_stride * chain, t + 1, io.stat_idx, io.alpha, a.th_out + a.ld_out * chain, a.g_out + a.ld_out * chain, eps, me.Minv,
                            chain, l, D);
@@ -702,7 +710,8 @@ static cudaError_t hmc_layout(const HmcArgs& a, cudaStream_t st, int G, int E) {
 }
 template <int MODEL, int FORM>
 static cudaError_t hmc_adapt_layout(const HmcArgs& a, cudaStream_t st, int G, int E) {
-    AHMC_DISPATCH_LAYOUT(launch_hmc_adapt_t, FORM, MODEL, AHMC_METRIC_DIAG);
+    // the metric the estimator adapts: Diag, or for WelfordCov the chain's own Dense rows
+    AHMC_DISPATCH_LAYOUT(launch_hmc_adapt_t, FORM, MODEL, FORM == AHMC_ADAPT_WELFORD_COV ? kMetricDenseChain : AHMC_METRIC_DIAG);
 }
 template <int FORM>
 static cudaError_t hmc_adapt_model(const HmcArgs& a, cudaStream_t st, int G, int E) {
@@ -733,19 +742,23 @@ static cudaError_t mom_layout(const MomentumArgs& a, cudaStream_t st, int G, int
 
 #define AHMC_DISPATCH_MM(FN, model_kind, metric_kind)                                                   \
     do {                                                                                                \
-        switch ((model_kind) * 3 + (metric_kind)) {                                                     \
+        switch ((model_kind) * 4 + (metric_kind)) {                                                     \
             case 0: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_UNIT>(a, st, G, E);                    \
             case 1: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG>(a, st, G, E);                    \
             case 2: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DENSE>(a, st, G, E);                   \
-            case 3: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);                    \
-            case 4: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);                    \
-            case 5: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);                   \
-            case 6: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);                   \
-            case 7: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);                   \
-            case 8: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);                  \
-            case 9: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT>(a, st, G, E);                        \
-            case 10: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG>(a, st, G, E);                       \
-            case 11: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DENSE>(a, st, G, E);                      \
+            case 3: return FN<AHMC_MODEL_STD_NORMAL, kMetricDenseChain>(a, st, G, E);                   \
+            case 4: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);                    \
+            case 5: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);                    \
+            case 6: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);                   \
+            case 7: return FN<AHMC_MODEL_DIAG_GAUSS, kMetricDenseChain>(a, st, G, E);                   \
+            case 8: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);                   \
+            case 9: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);                   \
+            case 10: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);                 \
+            case 11: return FN<AHMC_MODEL_DENSE_GAUSS, kMetricDenseChain>(a, st, G, E);                 \
+            case 12: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT>(a, st, G, E);                       \
+            case 13: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG>(a, st, G, E);                       \
+            case 14: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DENSE>(a, st, G, E);                      \
+            case 15: return FN<AHMC_MODEL_FUNNEL, kMetricDenseChain>(a, st, G, E);                      \
         }                                                                                               \
         return cudaErrorInvalidValue;                                                                   \
     } while (0)
@@ -760,10 +773,10 @@ cudaError_t launch_leapfrog(const LeapfrogArgs& a, cudaStream_t st, int* n_launc
     if (n_launches) *n_launches += 1;
     if (a.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
         const int cpb = kBlockThreads / G;
-        return user_launch((UserModule*)a.model.user, UK_LEAPFROG, a.metric.kind, G, E, &a, (unsigned)((a.N + cpb - 1) / cpb),
+        return user_launch((UserModule*)a.model.user, UK_LEAPFROG, metric_form(a.metric), G, E, &a, (unsigned)((a.N + cpb - 1) / cpb),
                            smem_bytes(AHMC_MODEL_USER, a.metric.kind, a.D, G), st);
     }
-    AHMC_DISPATCH_MM(lf_layout, a.model.kind, a.metric.kind);
+    AHMC_DISPATCH_MM(lf_layout, a.model.kind, metric_form(a.metric));
 }
 
 cudaError_t launch_find_eps(const FindEpsArgs& a, cudaStream_t st, int* n_launches) {
@@ -776,10 +789,10 @@ cudaError_t launch_find_eps(const FindEpsArgs& a, cudaStream_t st, int* n_launch
     if (n_launches) *n_launches += 1;
     if (a.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
         const int cpb = kBlockThreads / G;
-        return user_launch((UserModule*)a.model.user, UK_FIND_EPS, a.metric.kind, G, E, &a, (unsigned)((a.N + cpb - 1) / cpb),
+        return user_launch((UserModule*)a.model.user, UK_FIND_EPS, metric_form(a.metric), G, E, &a, (unsigned)((a.N + cpb - 1) / cpb),
                            smem_bytes(AHMC_MODEL_USER, a.metric.kind, a.D, G), st);
     }
-    AHMC_DISPATCH_MM(fe_layout, a.model.kind, a.metric.kind);
+    AHMC_DISPATCH_MM(fe_layout, a.model.kind, metric_form(a.metric));
 }
 
 cudaError_t launch_phasepoint(const PhasepointArgs& a, cudaStream_t st, int* n_launches) {
@@ -792,10 +805,10 @@ cudaError_t launch_phasepoint(const PhasepointArgs& a, cudaStream_t st, int* n_l
     if (n_launches) *n_launches += 1;
     if (a.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
         const int cpb = kBlockThreads / G;
-        return user_launch((UserModule*)a.model.user, UK_PHASEPOINT, a.metric.kind, G, E, &a, (unsigned)((a.N + cpb - 1) / cpb),
+        return user_launch((UserModule*)a.model.user, UK_PHASEPOINT, metric_form(a.metric), G, E, &a, (unsigned)((a.N + cpb - 1) / cpb),
                            smem_bytes(AHMC_MODEL_USER, a.metric.kind, a.D, G), st);
     }
-    AHMC_DISPATCH_MM(pp_layout, a.model.kind, a.metric.kind);
+    AHMC_DISPATCH_MM(pp_layout, a.model.kind, metric_form(a.metric));
 }
 
 cudaError_t launch_hmc(const HmcArgs& a, cudaStream_t st, int* n_launches) {
@@ -808,26 +821,28 @@ cudaError_t launch_hmc(const HmcArgs& a, cudaStream_t st, int* n_launches) {
     if (n_launches) *n_launches += 1;
     if (a.lf.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
         const int cpb = kBlockThreads / G;
-        return user_launch((UserModule*)a.lf.model.user, a.ad.enabled ? UK_HMC_ADAPT : UK_HMC, a.lf.metric.kind, G, E, &a,
+        return user_launch((UserModule*)a.lf.model.user, a.ad.enabled ? UK_HMC_ADAPT : UK_HMC, metric_form(a.lf.metric), G, E, &a,
                            (unsigned)((a.lf.N + cpb - 1) / cpb), smem_bytes(AHMC_MODEL_USER, a.lf.metric.kind, a.lf.D, G), st,
                            a.ad.enabled ? adapt_form(a.ad) : 0);
     }
-    if (a.ad.enabled) {  // the adaptive form: Diag metric only (the chain adapts its diagonal M^-1)
+    if (a.ad.enabled) {  // the adaptive forms: Diag metric (diagonal estimators) or Dense metric (WelfordCov form)
+        if (a.lf.metric.kind == AHMC_METRIC_DENSE) return hmc_adapt_model<AHMC_ADAPT_WELFORD_COV>(a, st, G, E);
         if (a.lf.metric.kind != AHMC_METRIC_DIAG) return cudaErrorInvalidValue;
         return adapt_form(a.ad) == AHMC_ADAPT_NUTPIE ? hmc_adapt_model<AHMC_ADAPT_NUTPIE>(a, st, G, E)
                                                      : hmc_adapt_model<AHMC_ADAPT_WELFORD>(a, st, G, E);
     }
-    AHMC_DISPATCH_MM(hmc_layout, a.lf.model.kind, a.lf.metric.kind);
+    AHMC_DISPATCH_MM(hmc_layout, a.lf.model.kind, metric_form(a.lf.metric));
 }
 
 cudaError_t launch_kick_drift(const SplitArgs& a, cudaStream_t st, int* n_launches) {
     int G, E;
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
-    switch (a.metric.kind) {
+    switch (metric_form(a.metric)) {
         case AHMC_METRIC_UNIT: return kd_layout<AHMC_METRIC_UNIT>(a, st, G, E);
         case AHMC_METRIC_DIAG: return kd_layout<AHMC_METRIC_DIAG>(a, st, G, E);
         case AHMC_METRIC_DENSE: return kd_layout<AHMC_METRIC_DENSE>(a, st, G, E);
+        case kMetricDenseChain: return kd_layout<kMetricDenseChain>(a, st, G, E);
     }
     return cudaErrorInvalidValue;
 }
@@ -835,10 +850,11 @@ cudaError_t launch_kick_energy(const SplitArgs& a, cudaStream_t st, int* n_launc
     int G, E;
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
-    switch (a.metric.kind) {
+    switch (metric_form(a.metric)) {
         case AHMC_METRIC_UNIT: return ke_layout<AHMC_METRIC_UNIT>(a, st, G, E);
         case AHMC_METRIC_DIAG: return ke_layout<AHMC_METRIC_DIAG>(a, st, G, E);
         case AHMC_METRIC_DENSE: return ke_layout<AHMC_METRIC_DENSE>(a, st, G, E);
+        case kMetricDenseChain: return ke_layout<kMetricDenseChain>(a, st, G, E);
     }
     return cudaErrorInvalidValue;
 }
@@ -857,10 +873,11 @@ cudaError_t launch_rand_momentum(const MomentumArgs& a, cudaStream_t st, int* n_
     }
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
-    switch (a.metric.kind) {
+    switch (metric_form(a.metric)) {
         case AHMC_METRIC_UNIT: return mom_layout<AHMC_METRIC_UNIT>(a, st, G, E);
         case AHMC_METRIC_DIAG: return mom_layout<AHMC_METRIC_DIAG>(a, st, G, E);
         case AHMC_METRIC_DENSE: return mom_layout<AHMC_METRIC_DENSE>(a, st, G, E);
+        case kMetricDenseChain: return mom_layout<kMetricDenseChain>(a, st, G, E);
     }
     return cudaErrorInvalidValue;
 }

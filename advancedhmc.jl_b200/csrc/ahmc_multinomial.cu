@@ -273,19 +273,23 @@ static cudaError_t mn_layout(const MultinomialArgs& a, cudaStream_t st, int G, i
 
 #define AHMC_MM(FN, mk, tk)                                                                   \
     do {                                                                                      \
-        switch ((mk) * 3 + (tk)) {                                                            \
-            case 0: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_UNIT>(a, st, G, E);          \
-            case 1: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG>(a, st, G, E);          \
-            case 2: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DENSE>(a, st, G, E);         \
-            case 3: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);          \
-            case 4: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);          \
-            case 5: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);         \
-            case 6: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);         \
-            case 7: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);         \
-            case 8: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);        \
-            case 9: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT>(a, st, G, E);              \
-            case 10: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG>(a, st, G, E);             \
-            case 11: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DENSE>(a, st, G, E);            \
+        switch ((mk) * 4 + (tk)) {                                                        \
+            case 0: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_UNIT>(a, st, G, E);      \
+            case 1: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG>(a, st, G, E);      \
+            case 2: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DENSE>(a, st, G, E);     \
+            case 3: return FN<AHMC_MODEL_STD_NORMAL, kMetricDenseChain>(a, st, G, E);     \
+            case 4: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);      \
+            case 5: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);      \
+            case 6: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);     \
+            case 7: return FN<AHMC_MODEL_DIAG_GAUSS, kMetricDenseChain>(a, st, G, E);     \
+            case 8: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);     \
+            case 9: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);     \
+            case 10: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);   \
+            case 11: return FN<AHMC_MODEL_DENSE_GAUSS, kMetricDenseChain>(a, st, G, E);   \
+            case 12: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT>(a, st, G, E);         \
+            case 13: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG>(a, st, G, E);         \
+            case 14: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DENSE>(a, st, G, E);        \
+            case 15: return FN<AHMC_MODEL_FUNNEL, kMetricDenseChain>(a, st, G, E);        \
         }                                                                                     \
         return cudaErrorInvalidValue;                                                         \
     } while (0)
@@ -294,13 +298,13 @@ cudaError_t launch_trajectory(const TrajArgs& a, cudaStream_t st, int* n_launche
     int G, E;
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
-    AHMC_MM(traj_layout, a.model.kind, a.metric.kind);
+    AHMC_MM(traj_layout, a.model.kind, metric_form(a.metric));
 }
 cudaError_t launch_multinomial(const MultinomialArgs& a, cudaStream_t st, int* n_launches) {
     int G, E;
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
-    AHMC_MM(mn_layout, a.model.kind, a.metric.kind);
+    AHMC_MM(mn_layout, a.model.kind, metric_form(a.metric));
 }
 
 #endif  // AHMC_SIMT_EMULATION

@@ -4,8 +4,8 @@
 
 namespace ahmc {
 
-long long nuts_scratch_doubles_per_chain(int D, int max_depth, int adapt_vectors) {
-    return nuts_level_doubles(D, max_depth) + (long long)adapt_vectors * D;
+long long nuts_scratch_doubles_per_chain(int D, int max_depth, long long adapt_doubles) {
+    return nuts_level_doubles(D, max_depth) + adapt_doubles;
 }
 
 // A (D x D, column-major) -> columns of leading dimension coop_lds(D), rows >= D zero: what the cooperative products stream
@@ -25,6 +25,7 @@ cudaError_t launch_pad_columns(const double* A, int D, double* out, cudaStream_t
 cudaError_t launch_nuts_variants(const NutsArgs& a, cudaStream_t st);  // ahmc_nuts_var.cu
 cudaError_t launch_nuts_adaptive(const NutsArgs& a, cudaStream_t st);  // ahmc_nuts_adapt.cu
 cudaError_t launch_nuts_nutpie(const NutsArgs& a, cudaStream_t st);    // ahmc_nuts_nutpie.cu
+cudaError_t launch_nuts_cov(const NutsArgs& a, cudaStream_t st);       // ahmc_nuts_cov.cu
 
 cudaError_t launch_nuts(const NutsArgs& a, cudaStream_t st, int* n_launches) {
     if (n_launches) *n_launches += 1;
@@ -35,9 +36,10 @@ cudaError_t launch_nuts(const NutsArgs& a, cudaStream_t st, int* n_launches) {
         const int cpb = kBlockThreads / G;
         const int maxd = a.max_depth > 0 ? a.max_depth : 1;
         const size_t sm = smem_bytes(AHMC_MODEL_USER, a.metric.kind, a.D, G) + (size_t)cpb * maxd * kLevelScalars * sizeof(double);
-        return user_launch((UserModule*)a.model.user, a.ad.enabled ? UK_NUTS_ADAPT : UK_NUTS, a.metric.kind, G, E, &a,
+        return user_launch((UserModule*)a.model.user, a.ad.enabled ? UK_NUTS_ADAPT : UK_NUTS, metric_form(a.metric), G, E, &a,
                            (unsigned)((a.N + cpb - 1) / cpb), sm, st, a.ad.enabled ? adapt_form(a.ad) : 0);
     }
+    if (a.ad.enabled && a.metric.kind == AHMC_METRIC_DENSE) return launch_nuts_cov(a, st);
     if (a.ad.enabled) return a.ad.adapt_metric == AHMC_ADAPT_NUTPIE ? launch_nuts_nutpie(a, st) : launch_nuts_adaptive(a, st);
     if (a.sampler != 0 || a.criterion != 0) return launch_nuts_variants(a, st);
     return nuts_dispatch<false, false, false>(a, st);

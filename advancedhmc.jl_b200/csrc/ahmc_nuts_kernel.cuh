@@ -20,9 +20,10 @@
 // Control flow is warp-uniform (`__any_sync` guarded blocks, per-group predicates) so that groups of
 // G < 32 lanes sharing a warp can sit at different tree positions while shuffles stay convergent.
 //
-// The kernel is compiled in three families, one translation unit each (build time): the default sampler/criterion
-// (ahmc_nuts.cu), the SliceTS / Classic / Strict variants (ahmc_nuts_var.cu), and the form that adapts step size and
-// diagonal metric per chain inside the launch (ahmc_nuts_adapt.cu).
+// The kernel is compiled in families, one translation unit each (build time): the default sampler/criterion
+// (ahmc_nuts.cu), the SliceTS / Classic / Strict variants (ahmc_nuts_var.cu), and the forms that adapt step size and
+// metric per chain inside the launch: diagonal WelfordVar (ahmc_nuts_adapt.cu), NutpieVar (ahmc_nuts_nutpie.cu) and, for
+// the Dense metric, WelfordCov (ahmc_nuts_cov.cu).
 #pragma once
 #include "ahmc_chain_adapt.cuh"
 
@@ -73,7 +74,9 @@ constexpr int nuts_min_blocks() { return E <= 4 ? 3 : (E <= 8 ? 2 : 1); }
 // (trajectory.jl:551-557, 579-613), selected at run time by a.sampler / a.criterion.
 //
 // ADAPT = 0: no adaptation; else the estimator form of the chain's in-launch adaptor (ahmc_chain_adapt.cuh):
-// AHMC_ADAPT_WELFORD (step size only or WelfordVar, by a.ad.adapt_metric) or AHMC_ADAPT_NUTPIE.
+// AHMC_ADAPT_WELFORD (step size only or WelfordVar, by a.ad.adapt_metric), AHMC_ADAPT_NUTPIE, or AHMC_ADAPT_WELFORD_COV
+// (METRIC = kMetricDenseChain: the chain's trajectories read its own M^-1 / factor rows, which its adaptor rewrites at
+// window ends).
 //
 // COOP = true (dense operators, one chain per warp, default family): the block has kCoopWarps warps and every D x D product
 // (dH/dr with a Dense metric, grad lp of a dense Gaussian) is a CTA-wide rendezvous -- the matrix is streamed from L2 into
@@ -81,10 +84,12 @@ constexpr int nuts_min_blocks() { return E <= 4 ? 3 : (E <= 8 ? 2 : 1); }
 // re-reading the whole matrix from L2 for its own chain (1.5 MB per leaf per chain at D = 256: the r01 kernel was L2-bound).
 // All warps of a block must then reach the product sites together: the votes that steer the loop around them are block-wide,
 // and a warp whose chain is idle or finished keeps taking part (its results are ignored, like idle groups of a warp).
+// A per-chain Dense metric (METRIC = kMetricDenseChain) never runs in this form: each warp reads its own matrices.
 // (the tile flag must not be called FULL: that is the namespace's all-lanes mask used by every *_sync below)
 template <int MODEL, int METRIC, int G, int E, bool VAR, int ADAPT, bool FULLTILE, bool COOP = false>
 __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 : nuts_min_blocks<E>()) nuts_kernel(const NutsArgs a) {
-    static_assert(!COOP || (G == 32 && !VAR), "COOP: one chain per warp, default family");
+    static_assert(!COOP || (G == 32 && !VAR && METRIC != kMetricDenseChain), "COOP: one chain per warp, default family, one matrix");
+    constexpr bool kCov = ADAPT == AHMC_ADAPT_WELFORD_COV;
     constexpr int kThreads = COOP ? kCoopThreads : kBlockThreads;
     // warp-uniform predicate -> uniform over everything that must stay in step (the warp, or the block when COOP)
     auto any_peer = [](bool p) -> bool {
@@ -93,7 +98,7 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
     };
     // Dense metric: a merge needs dH/dr = M^-1 r of the pending half's first leaf -- a D x D product.  The default family
     // caches the vector (slot 1 of the level holds M^-1 r_first instead of r_first) so merges do no dense product at all.
-    constexpr bool STORE_DR = !VAR && METRIC == AHMC_METRIC_DENSE;
+    constexpr bool STORE_DR = !VAR && is_dense_metric(METRIC);
     const int samp = VAR ? a.sampler : 0;    // 0 MultinomialTS, 1 SliceTS
     const int crit = VAR ? a.criterion : 0;  // 0 Generalised, 1 Classic, 2 StrictGeneralised
     double lu = 0.0;                         // SliceTS slice variable (log space)
@@ -105,7 +110,7 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
     const bool valid = chain0 < a.N;
     const long long chain = valid ? chain0 : a.N - 1;
     const int D = FULLTILE ? G * E : a.D;
-    const bool dense = (MODEL == AHMC_MODEL_DENSE_GAUSS) || (METRIC == AHMC_METRIC_DENSE) || (MODEL == AHMC_MODEL_USER);
+    const bool dense = (MODEL == AHMC_MODEL_DENSE_GAUSS) || is_dense_metric(METRIC) || (MODEL == AHMC_MODEL_USER);
     constexpr int kSlab = slab_vectors<MODEL>();
     double* xs = COOP ? smem : smem + (size_t)grp_in_block * kSlab * D;  // dense / user-target slab (unused otherwise)
     const int maxd = a.max_depth > 0 ? a.max_depth : 1;
@@ -130,13 +135,19 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
 
     double eps_c = a.eps_chain ? __ldg(a.eps_chain + chain) : a.eps;
     // adaptive family: the chain's adaptor (ahmc_chain_adapt.cuh), its estimator state behind the tree workspace
-    ChainAdapt<G, E, ADAPT == AHMC_ADAPT_NUTPIE ? AHMC_ADAPT_NUTPIE : AHMC_ADAPT_WELFORD> cad{};
+    ChainAdapt<G, E, ADAPT == AHMC_ADAPT_NUTPIE ? AHMC_ADAPT_NUTPIE : (kCov ? AHMC_ADAPT_WELFORD_COV : AHMC_ADAPT_WELFORD)> cad{};
     auto cad_ws = [&]() { return base + nuts_level_doubles(D, a.max_depth); };
 
     ModelOps<MODEL, G, E> mo;
     MetricOps<METRIC, G, E> me;
     mo.load(a.model, l, D);
-    me.load(a.metric, chain, l, D);
+    if constexpr (kCov) {  // the chain's own rows, filled before the first momentum draw
+        MetricDev rows;
+        cad.begin_dense(a.ad, a.metric, cad_ws(), valid, chain, l, D);
+        me.load(adapt_launch_metric<ADAPT>(a.metric, a.ad, D, rows), chain, l, D);
+    } else {
+        me.load(a.metric, chain, l, D);
+    }
     if constexpr (COOP) {
         mo.coop = smem;
         me.coop = smem;
@@ -270,7 +281,7 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
                 vstore<G, E>(RIGHT, s.th, l, D);
                 vstore<G, E>(RIGHT + D, s.r, l, D);
                 vstore<G, E>(RIGHT + 2 * (long long)D, s.g, l, D);
-                if constexpr (METRIC == AHMC_METRIC_DENSE) {  // M^-1 r0 (from the kinetic energy above) for both edges
+                if constexpr (is_dense_metric(METRIC)) {  // M^-1 r0 (from the kinetic energy above) for both edges
                     vstore<G, E>(LEFT_DR, drn, l, D);
                     vstore<G, E>(RIGHT_DR, drn, l, D);
                 }
@@ -278,7 +289,7 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
                 vstore<G, E>(a.th_out + a.ld_out * chain, s.th, l, D);
                 vstore<G, E>(a.r_out + a.ld_out * chain, s.r, l, D);
                 vstore<G, E>(a.g_out + a.ld_out * chain, s.g, l, D);
-                if (ADAPT && first) cad.begin(a.ad, cad_ws(), eps_c, me.Minv, chain, l, D);
+                if (ADAPT && first) cad.begin(a.ad, cad_ws(), eps_c, me.Minv, chain, l, D);  // (WelfordCov: the scalars only)
                 lw_tree = 0.0;
                 ww_tree = 1.0;
                 if (VAR && samp == 1) {  // SliceTS(rng, z0) = SliceTS(z0, neg_energy(z0) - randexp(rng), 1) (:144-145)
@@ -326,12 +337,18 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
                     if (st.tree_depth) st.tree_depth[si] = j;
                     if (st.numerical_error) st.numerical_error[si] = term_num ? 1 : 0;
                 }
-                if constexpr (ADAPT)  // iteration t + 1 of `sample` (sampler.jl:182): alpha = this transition's acceptance rate
+                if constexpr (ADAPT && !kCov)  // iteration t + 1 of `sample` (sampler.jl:182): alpha = this transition's acceptance rate
                     cad.update(a.ad, cad_ws(), t + 1, si, sa_tree / (double)na_tree, a.th_out + a.ld_out * chain, a.g_out + a.ld_out * chain,
                                eps_c, me.Minv, chain, l, D);
                 ++t;
                 if (t < a.n_transitions) need_init = true;
                 else finished = true;
+            }
+            if constexpr (kCov) {  // the WelfordCov form exchanges data across the group: every lane of the warp calls
+                // (a group that just finished a transition has advanced t: it was iteration t, entry (t - 1) * N + chain)
+                if (__any_sync(FULL, fin_now))
+                    cad.update_cov(a.ad, cad_ws(), fin_now, t, (long long)(t - 1) * a.N + chain, sa_tree / (double)na_tree,
+                                   a.th_out + a.ld_out * chain, eps_c, chain, l, D);
             }
         }
         if (any_peer(need_init)) continue;
@@ -670,7 +687,7 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
                 vstore<G, E>(edge + 2 * (long long)D, s.g, l, D);
                 vload_nc<G, E>(r_other, other + D, l, D);
             }
-            if constexpr (METRIC == AHMC_METRIC_DENSE) {  // dH/dr of both edges is parked: no product at the top level
+            if constexpr (is_dense_metric(METRIC)) {  // dH/dr of both edges is parked: no product at the top level
 #pragma unroll
                 for (int e = 0; e < E; ++e) t1[e] = 0.0;
                 if (complete) {
@@ -734,7 +751,8 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
 template <int MODEL, int METRIC, int G, int E, bool VAR, int ADAPT>
 static cudaError_t launch_nuts_v(const NutsArgs& a, cudaStream_t st) {
     const int maxd = a.max_depth > 0 ? a.max_depth : 1;
-    constexpr bool kDenseOps = MODEL == AHMC_MODEL_DENSE_GAUSS || METRIC == AHMC_METRIC_DENSE;
+    // (a per-chain Dense metric, kMetricDenseChain, has no shared matrix: it always runs warp per chain)
+    constexpr bool kDenseOps = (MODEL == AHMC_MODEL_DENSE_GAUSS || METRIC == AHMC_METRIC_DENSE) && METRIC != kMetricDenseChain;
     if constexpr (kDenseOps && G == 32 && !VAR) {
         // dense operators, one chain per warp: blocks of kCoopWarps chains share every D x D product (COOP form)
         const long long blocks = (a.N + kCoopWarps - 1) / kCoopWarps;
@@ -789,34 +807,41 @@ static cudaError_t nuts_layout(const NutsArgs& a, cudaStream_t st, int G, int E)
     return cudaErrorInvalidValue;
 }
 
-// model x metric dispatch of one (VAR, ADAPT) family (ADAPT: 0, or the adaptor's estimator form, ahmc_chain_adapt.cuh); DIAG_ONLY restricts the family to the Diag metric
-template <bool VAR, int ADAPT, bool DIAG_ONLY>
+// model x metric dispatch of one (VAR, ADAPT) family (ADAPT: 0, or the adaptor's estimator form, ahmc_chain_adapt.cuh);
+// ONE_METRIC restricts the family to the metric its estimator adapts: Diag, or Dense for WelfordCov
+template <bool VAR, int ADAPT, bool ONE_METRIC>
 static cudaError_t nuts_dispatch(const NutsArgs& a, cudaStream_t st) {
     int G, E;
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
-    if (DIAG_ONLY) {
-        if (a.metric.kind != AHMC_METRIC_DIAG) return cudaErrorInvalidValue;
+    if constexpr (ONE_METRIC) {  // (compile-time: the family holds no kernels for the other metrics)
+        // (WelfordCov: a Dense metric, shared or per chain, as the starting point; the launch reads the chain's own rows)
+        constexpr int MK = ADAPT == AHMC_ADAPT_WELFORD_COV ? kMetricDenseChain : AHMC_METRIC_DIAG;
+        if (a.metric.kind != (ADAPT == AHMC_ADAPT_WELFORD_COV ? AHMC_METRIC_DENSE : AHMC_METRIC_DIAG)) return cudaErrorInvalidValue;
         switch (a.model.kind) {
-            case AHMC_MODEL_STD_NORMAL: return nuts_layout<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
-            case AHMC_MODEL_DIAG_GAUSS: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
-            case AHMC_MODEL_DENSE_GAUSS: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
-            case AHMC_MODEL_FUNNEL: return nuts_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
+            case AHMC_MODEL_STD_NORMAL: return nuts_layout<AHMC_MODEL_STD_NORMAL, MK, VAR, ADAPT>(a, st, G, E);
+            case AHMC_MODEL_DIAG_GAUSS: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, MK, VAR, ADAPT>(a, st, G, E);
+            case AHMC_MODEL_DENSE_GAUSS: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, MK, VAR, ADAPT>(a, st, G, E);
+            case AHMC_MODEL_FUNNEL: return nuts_layout<AHMC_MODEL_FUNNEL, MK, VAR, ADAPT>(a, st, G, E);
         }
         return cudaErrorInvalidValue;
     } else {
-        switch (a.model.kind * 3 + a.metric.kind) {
+        switch (a.model.kind * 4 + metric_form(a.metric)) {
             case 0: return nuts_layout<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
             case 1: return nuts_layout<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
             case 2: return nuts_layout<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
-            case 3: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
-            case 4: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
-            case 5: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
-            case 6: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
-            case 7: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
-            case 8: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
-            case 9: return nuts_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
-            case 10: return nuts_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
-            case 11: return nuts_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
+            case 3: return nuts_layout<AHMC_MODEL_STD_NORMAL, kMetricDenseChain, VAR, ADAPT>(a, st, G, E);
+            case 4: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
+            case 5: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
+            case 6: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
+            case 7: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, kMetricDenseChain, VAR, ADAPT>(a, st, G, E);
+            case 8: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
+            case 9: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
+            case 10: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
+            case 11: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, kMetricDenseChain, VAR, ADAPT>(a, st, G, E);
+            case 12: return nuts_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
+            case 13: return nuts_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
+            case 14: return nuts_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
+            case 15: return nuts_layout<AHMC_MODEL_FUNNEL, kMetricDenseChain, VAR, ADAPT>(a, st, G, E);
         }
         return cudaErrorInvalidValue;
     }

@@ -76,7 +76,13 @@ typedef struct ahmc_model ahmc_model;
 /* Metric descriptor.  `Minv`: Diag -> D entries (chain_stride 0) or D x N per-chain (chain_stride = D,
  * metric.jl:64); Dense -> D x D column-major.  `cholU`: Dense only, upper factor of cholesky(Minv)
  * (metric.jl:104-109), needed by ahmc_rand_momentum_f64 and the transition kernels.  Device pointers
- * (host pointers with AHMC_FLAG_HOST_BUFFERS). */
+ * (host pointers with AHMC_FLAG_HOST_BUFFERS).
+ * Per-chain Dense (D <= 512; the D x D x N form `DenseEuclideanMetric{..., AbstractArray{T,3}}`, metric.jl:89-103):
+ * chain_stride >= D*D puts chain c's M^-1 at Minv + chain_stride*c and its factor at cholU + chain_stride*c (both
+ * column-major D x D; only the factor's upper triangle is read); chain_stride = 0 is the one shared matrix and
+ * 0 < chain_stride < D*D is AHMC_ERR_INVALID.  Every Dense entry point accepts it.  Calls that share one matrix across
+ * the chains of a block (the cooperative NUTS form, the tiled trajectory kernel) are then replaced by their warp-per-chain
+ * forms, which read each chain's matrices from global memory: D^2 doubles per dense product per chain. */
 typedef struct ahmc_metric {
     int32_t kind;
     const double* Minv;
@@ -264,9 +270,20 @@ int ahmc_nuts_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metr
  * D x N variance, i.e. a per-chain diagonal M^-1), scheduled like `StanHMCAdaptor` (stan_adaptor.jl:13-50, 137-159: windows, reset of both
  * adaptors at each window end, `finalize!` eps = exp(x_bar) after iteration n_adapts).  Because nothing is pooled,
  * chains never wait for each other: iterations 1..n_adapts adapt, n_adapts+1..n_transitions sample with the final
- * eps / M^-1.  Requires the Diag metric (shared or per-chain M^-1 as the starting point), MultinomialTS +
- * GeneralisedNoUTurn, Philox randomness (no tapes).  Deviation from the reference: a non-finite eps proposal reverts
- * that chain only (the reference reverts every chain, "buggy for batch mode" by its own comment, stepsize.jl:199-203). */
+ * eps / M^-1.  Requires the Diag metric (shared or per-chain M^-1 as the starting point) or, on built-in targets, the
+ * Dense metric (shared or per chain) with AHMC_ADAPT_STEPSIZE or AHMC_ADAPT_WELFORD_COV; MultinomialTS +
+ * GeneralisedNoUTurn, Philox randomness (no tapes).  Dense with WelfordVar / NutpieVar, and Dense on run-time compiled
+ * targets: AHMC_ERR_UNSUPPORTED; AHMC_ADAPT_WELFORD_COV with a Unit or Diag metric: AHMC_ERR_INVALID.
+ * With AHMC_ADAPT_WELFORD_COV chain c behaves like `sample(h_c, NUTS, n; adaptor = StanHMCAdaptor(WelfordCov(D),
+ * NesterovDualAveraging(delta, eps_c)))`: the launch copies the starting metric into the chain's Minv_chain / cholU_chain
+ * rows, every trajectory reads those rows, and each window end with n >= n_min rewrites them.  Estimator workspace:
+ * D + D^2 doubles per chain (mean and the full matrix M).  With AHMC_ADAPT_STEPSIZE and a Dense metric the rows are
+ * optional (given: both, they receive the starting metric and are what the launch reads).  n_adapts = 0 gives
+ * ahmc_nuts_sample_f64 / ahmc_hmc_sample_f64 with the per-chain Dense metric of the rows bit for bit.
+ * Deviations from the reference: a non-finite eps proposal reverts that chain only (the reference reverts every chain,
+ * "buggy for batch mode" by its own comment, stepsize.jl:199-203); a WelfordCov estimate whose Cholesky factorisation meets
+ * a non-positive or non-finite pivot (rounding, or non-finite draws) leaves that chain's previous M^-1 and factor in place
+ * (the reference throws PosDefException). */
 typedef struct ahmc_adapt_cfg {
     int32_t n_adapts;                             /* 0 <= n_adapts <= n_transitions */
     int32_t init_buffer, term_buffer, window_size; /* Stan defaults 75 / 50 / 25; a schedule with more than 12 window
@@ -277,12 +294,18 @@ typedef struct ahmc_adapt_cfg {
     double* eps_chain;  /* N, in: initial step size per chain; out: adapted step size per chain */
     double* Minv_chain; /* N x D, out: adapted diagonal M^-1 per chain (required iff adapt_metric != 0) */
     double* eps_trace;  /* nullable, n_transitions x N: the step size each transition used (`step_size` stat) */
+    double* cholU_chain; /* WelfordCov: N x D x D, out (required): the upper Cholesky factor of each chain's adapted M^-1
+                            (appended last: the offsets of the fields above are those of earlier versions) */
 } ahmc_adapt_cfg;
 /* ahmc_adapt_cfg.adapt_metric: the per-chain metric estimator */
 #define AHMC_ADAPT_STEPSIZE 0 /* step size only: M^-1 stays the metric's */
 #define AHMC_ADAPT_WELFORD 1  /* WelfordVar((D, N)) of the positions (massmatrix.jl:141-157) */
 #define AHMC_ADAPT_NUTPIE 2   /* NutpieVar((D, N)) of positions and gradients (massmatrix.jl:172-250):
                                  M^-1 = sqrt(var(theta) / var(grad log pi)), each variance regularised as WelfordVar's */
+#define AHMC_ADAPT_WELFORD_COV 3 /* Dense metric only: one WelfordCov(D) per chain (massmatrix.jl:284-340); at a window end
+                                    M^-1 = n/((n+5)(n-1)) M + 1e-3 * 5/(n+5) I and its upper Cholesky factor (of the upper
+                                    triangle, `cholesky(Symmetric(M^-1)).U`, metric.jl:105-120) replace the chain's
+                                    Minv_chain / cholU_chain rows (N x D x D each), which the chain's trajectories read */
 int ahmc_nuts_adapt_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, int32_t D, int64_t N,
                                int32_t max_depth, double delta_max, int32_t n_transitions, const ahmc_adapt_cfg* cfg,
                                const ahmc_rng* rng, const ahmc_phasepoint* z_in, const ahmc_phasepoint* z_out,

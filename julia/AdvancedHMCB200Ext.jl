@@ -68,6 +68,7 @@ struct CAdaptCfg
     delta::Float64; gamma::Float64; t0::Float64; kappa::Float64
     adapt_metric::Int32; n_min::Int32
     eps_chain::Ptr{Float64}; Minv_chain::Ptr{Float64}; eps_trace::Ptr{Float64}
+    cholU_chain::Ptr{Float64}  # AHMC_ADAPT_WELFORD_COV (adapt_metric = 3): N x D x D upper factors, out
 end
 struct CPooledCfg
     n_adapts::Int32; init_buffer::Int32; term_buffer::Int32; window_size::Int32
@@ -206,8 +207,13 @@ temper_alpha(lf::B200Leapfrog) = lf.α
 
 cmetric(m::UnitEuclideanMetric, N) = CMetric(0, C_NULL, 0, C_NULL)
 cmetric(m::DiagEuclideanMetric, N) = CMetric(1, dptr(m.M⁻¹), ndims(m.M⁻¹) == 2 ? size(m.M⁻¹, 1) : 0, C_NULL)
-# Dense: the caller keeps `U = CuArray(Matrix(m.cholM⁻¹))` alive for the duration of the call
+# Dense: the caller keeps `U = CuArray(Matrix(m.cholM⁻¹))` alive for the duration of the call.
+# The 3-d form `DenseEuclideanMetric{T,AV,<:AbstractArray{T,3}}` (metric.jl:89-103, D x D x N: chain c's M⁻¹ is
+# M⁻¹[:, :, c]) is the per-chain Dense metric of the C ABI: chain_stride = D*D, and U is a D x D x N CuArray of the chains'
+# upper factors (`cat(cholesky(Symmetric(M⁻¹[:, :, c])).U... ; dims = 3)`, or the cholU_chain output of an in-launch
+# WelfordCov warm-up, which needs no refactorisation).
 cmetric(m::DenseEuclideanMetric, N, U::CuMatrix{Float64}) = CMetric(2, dptr(m.M⁻¹), 0, dptr(U))
+cmetric(m::DenseEuclideanMetric, N, U::CuArray{Float64,3}) = CMetric(2, dptr(m.M⁻¹), size(U, 1) * size(U, 2), dptr(U))
 dense_factor(m::DenseEuclideanMetric) = CuArray(Matrix(m.cholM⁻¹))
 dense_factor(m) = nothing
 metric_desc(m::DenseEuclideanMetric, N, U) = cmetric(m, N, U)
