@@ -23,6 +23,12 @@
 
 using namespace ahmc;
 
+// a grow-only device buffer of the context (see ensure)
+struct DevBuf {
+    void* p = nullptr;
+    size_t bytes = 0;
+};
+
 struct ahmc_ctx {
     int device = 0;
     int sm_count = 0;  // streaming multiprocessors of the device (grid size of the one-wave reductions)
@@ -31,20 +37,13 @@ struct ahmc_ctx {
     std::string err;
     int64_t launches = 0;
     int* d_min_break = nullptr;   // device int for COMPAT_BREAK_ALL
-    char* arena = nullptr;        // grow-only device arena used by HOST_BUFFERS staging
-    size_t arena_bytes = 0;
-    double* nuts_scratch = nullptr;  // per-chain NUTS tree workspace
-    size_t nuts_scratch_bytes = 0;
-    double* adapt_scratch = nullptr;
-    size_t adapt_scratch_bytes = 0;
-    double* mn_scratch = nullptr;  // multinomial-static per-chain energy tape
-    size_t mn_scratch_bytes = 0;
-    char* dense_scratch = nullptr;  // K4: padded Minv, norms, per-chain fallback mask
-    double* coop_scratch = nullptr;  // cooperative NUTS products: Minv and cholU with padded columns (coop_lds)
-    size_t coop_scratch_doubles = 0;
-    size_t dense_scratch_bytes = 0;
-    char* split_scratch = nullptr;   // callback (split-step) mode workspace
-    size_t split_scratch_bytes = 0;
+    DevBuf arena;         // HOST_BUFFERS staging
+    DevBuf chain_ws;      // per-chain workspace: NUTS trees, in-launch adaptors' estimators, D > 512 start points
+    DevBuf summary_ws;    // adapt_summary: block partials and the completion counter
+    DevBuf energy_ws;     // multinomial-static per-chain energy tape
+    DevBuf dense_ws;      // K4: padded Minv, norms, per-chain fallback mask
+    DevBuf coop_ws;       // cooperative NUTS products: Minv and cholU with padded columns (coop_lds)
+    DevBuf split_ws;      // callback (split-step) mode workspace
     // host-buffer pipeline: H2D stream, compute stream (= stream), D2H stream, one event pair per chunk
     static constexpr int kMaxPipeChunks = 32, kPipeStreams = 5;  // 3 upload, 1 download, 1 second compute
     cudaStream_t pipe[kPipeStreams] = {};
@@ -115,68 +114,89 @@ struct DeviceGuard {
     }
 };
 
-// Maps caller arrays to device arrays.  Device-pointer mode: identity.  HOST_BUFFERS mode: bump-allocates
-// from the context arena, copies inputs host->device on the context stream and outputs device->host in finish().
+// grows `b` to at least `need` bytes; the old contents are not kept.  Work already enqueued may still use the old
+// allocation, so the context's streams are drained first (the pipeline streams are idle between calls).
+int ensure(ahmc_ctx* ctx, DevBuf& b, size_t need, const char* what) {
+    if (need <= b.bytes) return AHMC_OK;
+    CU(cudaStreamSynchronize(ctx->stream));
+    for (cudaStream_t s : ctx->pipe)
+        if (s) CU(cudaStreamSynchronize(s));
+    CU(cudaFree(b.p));
+    b.p = nullptr;
+    b.bytes = 0;
+    cudaError_t e = cudaMalloc(&b.p, need);
+    if (e != cudaSuccess) {
+        b.p = nullptr;
+        return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for %s failed: %s", need, what, cudaGetErrorString(e));
+    }
+    b.bytes = need;
+    return AHMC_OK;
+}
+// the staging arena keeps 25 % headroom, so that a run of slowly growing calls does not reallocate every time
+int ensure_arena(ahmc_ctx* ctx, size_t need) {
+    return need > ctx->arena.bytes ? ensure(ctx, ctx->arena, need + need / 4, "staging") : AHMC_OK;
+}
+
+// Lays arrays out back to back, each on a 256-byte boundary.  Over base == nullptr it only measures (every pointer it
+// hands out is nullptr), so one layout function gives both the size of a buffer and its pointers.
+struct Carver {
+    char* base = nullptr;
+    size_t off = 0;
+    template <class T>
+    T* take(size_t count, bool want = true) {  // `want` false: nullptr, nothing taken
+        if (!want) return nullptr;
+        T* p = base ? (T*)(base + off) : nullptr;
+        off += (count * sizeof(T) + 255) & ~(size_t)255;
+        return p;
+    }
+};
+// grows `b` to the size of `layout` (a function of Carver&) and runs it over `b`
+template <class Layout>
+int carve(ahmc_ctx* ctx, DevBuf& b, const char* what, Layout&& layout) {
+    Carver m;
+    layout(m);
+    int rc = ensure(ctx, b, m.off, what);
+    if (rc) return rc;
+    Carver c{(char*)b.p};
+    layout(c);
+    return AHMC_OK;
+}
+
+// Maps caller arrays to device arrays.  An entry point describes its arrays once, in a bind function (of Stager&) that
+// calls in / out / inout for each and that neither launches kernels nor reads staged data; stage() runs it.
+// Device-pointer mode: one pass, the identity.  HOST_BUFFERS mode: a first pass only measures the arrays, the context
+// arena grows to fit, and a second pass carves them out of it and enqueues the uploads on the context stream;
+// finish() enqueues the downloads.  The first failed copy is kept and returned by stage().
 class Stager {
 public:
     Stager(ahmc_ctx* c, bool host) : ctx_(c), host_(host) {}
-    // first pass: reserve; second pass: bind.  (two passes so the arena is sized before any copy)
-    size_t need = 0;
-    // `bytes` may cover several arrays that are later carved one by one (each rounded up to 256 B on its own):
-    // kSlack pays for those roundings (every call site stages fewer than kSlack / 256 arrays)
-    static constexpr size_t kSlack = 64 * 256;
-    void reserve(size_t bytes) { need += (bytes + 255) & ~(size_t)255; }
-    int prepare() {
-        if (!host_) return AHMC_OK;
-        ahmc_ctx* ctx = ctx_;
-        need += kSlack;
-        if (need > ctx->arena_bytes) {
-            if (ctx->arena) {
-                CU(cudaStreamSynchronize(ctx->stream));
-                CU(cudaFree(ctx->arena));
-                ctx->arena = nullptr;
-                ctx->arena_bytes = 0;
-            }
-            size_t cap = need + need / 4;
-            cudaError_t e = cudaMalloc((void**)&ctx->arena, cap);
-            if (e != cudaSuccess) return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for staging failed: %s", cap, cudaGetErrorString(e));
-            ctx->arena_bytes = cap;
+    template <class Bind>
+    int stage(Bind&& bind) {
+        if (!host_) {
+            bind(*this);
+            return AHMC_OK;
         }
-        off_ = 0;
-        return AHMC_OK;
+        sizing_ = true;
+        carver_ = Carver{};
+        bind(*this);
+        sizing_ = false;
+        int rc = ensure_arena(ctx_, carver_.off);
+        if (rc) return rc;
+        carver_ = Carver{(char*)ctx_->arena.p};
+        bind(*this);
+        return rc_;
     }
     template <class T>
-    int in(const T* h, size_t count, const T** d) {
-        if (!h) { *d = nullptr; return AHMC_OK; }
-        if (!host_) { *d = h; return AHMC_OK; }
-        ahmc_ctx* ctx = ctx_;
-        T* p = (T*)alloc(count * sizeof(T));
-        if (!p) return overflow();
-        CU(cudaMemcpyAsync(p, h, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-        *d = p;
-        return AHMC_OK;
+    void in(const T* h, size_t count, const T** d) {
+        *d = map(h, count, true, false);
     }
     template <class T>
-    int out(T* h, size_t count, T** d) {
-        if (!h) { *d = nullptr; return AHMC_OK; }
-        if (!host_) { *d = h; return AHMC_OK; }
-        T* p = (T*)alloc(count * sizeof(T));
-        if (!p) return overflow();
-        outs_.push_back({(void*)h, (void*)p, count * sizeof(T)});
-        *d = p;
-        return AHMC_OK;
+    void out(T* h, size_t count, T** d) {
+        *d = map(h, count, false, true);
     }
     template <class T>
-    int inout(T* h, size_t count, T** d) {  // copied in now, copied back at finish
-        if (!h) { *d = nullptr; return AHMC_OK; }
-        if (!host_) { *d = h; return AHMC_OK; }
-        ahmc_ctx* ctx = ctx_;
-        T* p = (T*)alloc(count * sizeof(T));
-        if (!p) return overflow();
-        CU(cudaMemcpyAsync(p, h, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-        outs_.push_back({(void*)h, (void*)p, count * sizeof(T)});
-        *d = p;
-        return AHMC_OK;
+    void inout(T* h, size_t count, T** d) {  // copied in now, copied back at finish
+        *d = map(h, count, true, true);
     }
     int finish() {
         ahmc_ctx* ctx = ctx_;
@@ -187,17 +207,25 @@ public:
 
 private:
     struct Out { void* h; void* d; size_t bytes; };
-    void* alloc(size_t bytes) {  // nullptr when the reservation pass undercounted: never hand out memory past the arena
-        const size_t b = (bytes + 255) & ~(size_t)255;
-        if (off_ + b > ctx_->arena_bytes) return nullptr;
-        void* p = ctx_->arena + off_;
-        off_ += b;
+    template <class T>
+    T* map(T* h, size_t count, bool upload, bool download) {
+        if (!h || !host_) return h;
+        T* p = (T*)carver_.take<T>(count);
+        if (sizing_) return p;
+        if (upload && !rc_) rc_ = upload_now((void*)p, h, count * sizeof(T));
+        if (download) outs_.push_back({(void*)h, (void*)p, count * sizeof(T)});
         return p;
     }
-    int overflow() { return fail(ctx_, AHMC_ERR_NOMEM, "internal: host-buffer staging arena undersized (%zu of %zu bytes used)", off_, ctx_->arena_bytes); }
+    int upload_now(void* d, const void* h, size_t bytes) {
+        ahmc_ctx* ctx = ctx_;
+        CU(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, ctx->stream));
+        return AHMC_OK;
+    }
     ahmc_ctx* ctx_;
     bool host_;
-    size_t off_ = 0;
+    bool sizing_ = false;
+    Carver carver_;
+    int rc_ = AHMC_OK;
     std::vector<Out> outs_;
 };
 
@@ -267,19 +295,36 @@ bool per_chain_dense(const ahmc_metric* m) { return m->kind == AHMC_METRIC_DENSE
 ModelDev model_dev(const ahmc_model* m) { return ModelDev{m->kind, m->D, m->d_p0, m->d_p1, m->c0, m->rtc, m->d_p1_coop}; }
 
 // stage the metric descriptor (device or host pointers) into a MetricDev
-int stage_metric(Stager& st, const ahmc_metric* m, int32_t D, int64_t N, MetricDev* out) {
+void stage_metric(Stager& st, const ahmc_metric* m, int32_t D, int64_t N, MetricDev* out) {
     out->kind = m->kind;
     out->chain_stride = m->kind != AHMC_METRIC_UNIT ? m->chain_stride : 0;
     out->Minv_coop = nullptr;
     out->cholU_coop = nullptr;
-    int rc = st.in(m->Minv, metric_minv_count(m, D, N), &out->Minv);
-    if (rc) return rc;
+    st.in(m->Minv, metric_minv_count(m, D, N), &out->Minv);
     // a Dense factor has the layout of its M^-1 (shared, or per chain at the same stride)
-    return st.in(m->kind == AHMC_METRIC_DENSE ? m->cholU : (const double*)nullptr, metric_minv_count(m, D, N), &out->cholU);
+    st.in(m->kind == AHMC_METRIC_DENSE ? m->cholU : (const double*)nullptr, metric_minv_count(m, D, N), &out->cholU);
 }
-void reserve_metric(Stager& st, const ahmc_metric* m, int32_t D, int64_t N) {
-    st.reserve(metric_minv_count(m, D, N) * sizeof(double));
-    if (m->kind == AHMC_METRIC_DENSE) st.reserve(metric_minv_count(m, D, N) * sizeof(double));
+
+// the phase-point fields the argument blocks share by name.  In: theta, r, -grad lp[, lp] of z (N chains).
+template <class Args>
+void stage_pp_in(Stager& st, const ahmc_phasepoint* z, int64_t N, Args& a, const double** lp_in = nullptr) {
+    const size_t c = (size_t)z->ld * N;
+    a.ld_in = z->ld;
+    st.in((const double*)z->theta, c, &a.th_in);
+    st.in((const double*)z->r, c, &a.r_in);
+    st.in((const double*)z->lp_gradient, c, &a.g_in);
+    if (lp_in) st.in((const double*)z->lp_value, (size_t)N, lp_in);
+}
+// Out: `nv` doubles per vector field (ld * N, or a whole trajectory), `ns` per energy[, dH/dr from lk_gradient]
+template <class Args>
+void stage_pp_out(Stager& st, const ahmc_phasepoint* z, size_t nv, size_t ns, Args& a, double** dr_out = nullptr) {
+    a.ld_out = z->ld;
+    st.out(z->theta, nv, &a.th_out);
+    st.out(z->r, nv, &a.r_out);
+    st.out(z->lp_gradient, nv, &a.g_out);
+    if (dr_out) st.out(z->lk_gradient, nv, dr_out);
+    st.out(z->lp_value, ns, &a.lp_out);
+    st.out(z->lk_value, ns, &a.lk_out);
 }
 
 int finish_call(ahmc_ctx* ctx, Stager& st, uint32_t flags) {
@@ -302,27 +347,15 @@ struct SplitWork {
 };
 
 int split_workspace(ahmc_ctx* ctx, int32_t D, int64_t N, int64_t ld, SplitWork* w) {
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t need = al((size_t)N * 8) + al((size_t)ld * N * 8) + al((size_t)D * N * 8) + al((size_t)N * 8) +
-                        al((size_t)N * 4) * 2 + 256;
-    if (need > ctx->split_scratch_bytes) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->split_scratch);
-        ctx->split_scratch = nullptr;
-        ctx->split_scratch_bytes = 0;
-        if (cudaMalloc((void**)&ctx->split_scratch, need) != cudaSuccess)
-            return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for the split-step workspace failed", need);
-        ctx->split_scratch_bytes = need;
-    }
-    char* p = ctx->split_scratch;
-    w->cb_lp = (double*)p; p += al((size_t)N * 8);
-    w->cb_grad = (double*)p; p += al((size_t)ld * N * 8);
-    w->r0 = (double*)p; p += al((size_t)D * N * 8);
-    w->lk0 = (double*)p; p += al((size_t)N * 8);
-    w->status = (uint32_t*)p; p += al((size_t)N * 4);
-    w->steps = (int32_t*)p; p += al((size_t)N * 4);
-    w->flag = (int*)p;
-    return AHMC_OK;
+    return carve(ctx, ctx->split_ws, "the split-step workspace", [&](Carver& c) {
+        w->cb_lp = c.take<double>((size_t)N);
+        w->cb_grad = c.take<double>((size_t)ld * N);
+        w->r0 = c.take<double>((size_t)D * N);
+        w->lk0 = c.take<double>((size_t)N);
+        w->status = c.take<uint32_t>((size_t)N);
+        w->steps = c.take<int32_t>((size_t)N);
+        w->flag = c.take<int>(1);
+    });
 }
 
 // user closure on the context stream: lp[N], grad[D x N] <- theta
@@ -371,6 +404,17 @@ int split_trajectory(ahmc_ctx* ctx, const ahmc_model* model, const MetricDev& md
     return AHMC_OK;
 }
 
+// can the tiled DMMA trajectory (K4) run this target and metric?  A Gaussian target with a GEMM-shaped operator (dense
+// metric and/or dense-Gaussian target), one M^-1 shared by all chains, no EXACT_CHECKS, and a tile shape for D
+bool dense_tile_eligible(const ahmc_model* model, const MetricDev& metric, uint32_t flags, int32_t D) {
+    const bool gauss = model->kind == AHMC_MODEL_STD_NORMAL || model->kind == AHMC_MODEL_DIAG_GAUSS ||
+                       model->kind == AHMC_MODEL_DENSE_GAUSS;
+    const bool has_dense = model->kind == AHMC_MODEL_DENSE_GAUSS || metric.kind == AHMC_METRIC_DENSE;
+    int Dp, RB, CB;
+    return gauss && has_dense && metric.chain_stride == 0 && !(flags & AHMC_FLAG_EXACT_CHECKS) &&
+           dense_tile_shape(D, &Dp, &RB, &CB) && (model->kind != AHMC_MODEL_DENSE_GAUSS || model->d_p1_pad);
+}
+
 // K4 dispatch: GEMM-shaped operators (dense metric and/or dense-Gaussian target) -> tiled DMMA kernel; chains of tiles it
 // declines (magnitude proof not met) are redone by the exact warp-per-chain kernel from the untouched inputs.
 // `a` holds DEVICE pointers.  Returns 1 if handled, 0 if the configuration is not eligible, < 0 on error.
@@ -378,28 +422,17 @@ int try_dense_trajectory(ahmc_ctx* ctx, const ahmc_model* model, LeapfrogArgs& a
                          bool compat, int* nl) {
     const int D = a.D;
     const long long N = a.N;
-    const bool gauss = model->kind == AHMC_MODEL_STD_NORMAL || model->kind == AHMC_MODEL_DIAG_GAUSS ||
-                       model->kind == AHMC_MODEL_DENSE_GAUSS;
-    const bool metric_ok = a.metric.chain_stride == 0;  // the tile kernel shares one M^-1 across its chains
-    const bool has_dense = model->kind == AHMC_MODEL_DENSE_GAUSS || a.metric.kind == AHMC_METRIC_DENSE;
+    if (!dense_tile_eligible(model, a.metric, a.flags, D) || compat || !a.g_in || temper_alpha > 0.0) return 0;
     int Dp, RB, CB;
-    if (!(gauss && metric_ok && has_dense && !compat && a.g_in && !(a.flags & AHMC_FLAG_EXACT_CHECKS) && !(temper_alpha > 0.0) &&
-          dense_tile_shape(D, &Dp, &RB, &CB) && (model->kind != AHMC_MODEL_DENSE_GAUSS || model->d_p1_pad)))
-        return 0;
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t need = al(dense_mat_doubles(Dp) * 8) + al(16) + al((size_t)N);
-    if (need > ctx->dense_scratch_bytes) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->dense_scratch);
-        ctx->dense_scratch = nullptr;
-        ctx->dense_scratch_bytes = 0;
-        if (cudaMalloc((void**)&ctx->dense_scratch, need) != cudaSuccess)
-            return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for the dense workspace failed", need);
-        ctx->dense_scratch_bytes = need;
-    }
-    double* Mpad = (double*)ctx->dense_scratch;
-    double* norms = (double*)(ctx->dense_scratch + al(dense_mat_doubles(Dp) * 8));
-    uint8_t* mask = (uint8_t*)(ctx->dense_scratch + al(dense_mat_doubles(Dp) * 8) + al(16));
+    dense_tile_shape(D, &Dp, &RB, &CB);
+    double *Mpad, *norms;
+    uint8_t* mask;
+    int rc = carve(ctx, ctx->dense_ws, "the dense workspace", [&](Carver& c) {
+        Mpad = c.take<double>(dense_mat_doubles(Dp));
+        norms = c.take<double>(2);
+        mask = c.take<uint8_t>((size_t)N);
+    });
+    if (rc) return rc;
     DenseTrajHost h{};
     h.D = D; h.Dp = Dp; h.N = N; h.c0 = model->c0;
     h.mu = (model->kind == AHMC_MODEL_STD_NORMAL) ? nullptr : model->d_p0;
@@ -432,6 +465,50 @@ int try_dense_trajectory(ahmc_ctx* ctx, const ahmc_model* model, LeapfrogArgs& a
     b.min_break = nullptr;
     CU(launch_leapfrog(b, ctx->stream, nl));
     return 1;
+}
+// hmc_kernel's transition, unfused, for what it cannot run itself (callback targets, the tiled DMMA trajectory):
+// refresh -> kinetic energy -> start point into z_out -> `trajectory(w)` in place on z_out (< 0 on error) -> MH select.
+// `h` holds DEVICE pointers.
+template <class Trajectory>
+static int unfused_transition(ahmc_ctx* ctx, const HmcArgs& h, int* nl, Trajectory&& trajectory) {
+    const LeapfrogArgs& a = h.lf;
+    const int D = a.D;
+    const long long N = a.N;
+    SplitWork w;
+    int rc = split_workspace(ctx, D, N, a.ld_out, &w);
+    if (rc) return rc;
+    if (h.refresh) {
+        MomentumArgs ma{};
+        ma.metric = a.metric; ma.D = D; ma.N = N; ma.seed = h.rng.seed; ma.offset = h.rng.offset;
+        ma.normal_tape = h.rng.normal_tape; ma.r = w.r0; ma.ld = D;
+        CU(launch_rand_momentum(ma, ctx->stream, nl));
+    } else {
+        CU(cudaMemcpy2DAsync(w.r0, (size_t)D * 8, a.r_in, (size_t)a.ld_in * 8, (size_t)D * 8, (size_t)N,
+                             cudaMemcpyDeviceToDevice, ctx->stream));
+    }
+    SplitArgs k0{};  // lk0 = neg kinetic energy of the refreshed momentum
+    k0.metric = a.metric; k0.D = D; k0.N = N; k0.fwd = 1; k0.mul = 1.0; k0.no_kick = 1;
+    k0.r = w.r0; k0.lk = w.lk0; k0.ld = D;
+    CU(launch_kick_energy(k0, ctx->stream, nl));
+    auto cp = [&](double* dst, const double* src, int64_t lds) -> cudaError_t {
+        if (dst == src) return cudaSuccess;
+        return cudaMemcpy2DAsync(dst, (size_t)a.ld_out * 8, src, (size_t)lds * 8, (size_t)D * 8, (size_t)N,
+                                 cudaMemcpyDeviceToDevice, ctx->stream);
+    };
+    if (a.th_out == a.th_in)
+        return fail(ctx, AHMC_ERR_INVALID, "callback-mode transitions need z_out distinct from z_in (the start point is re-read on rejection)");
+    CU(cp(a.th_out, a.th_in, a.ld_in));
+    CU(cp(a.g_out, a.g_in, a.ld_in));
+    CU(cp(a.r_out, w.r0, D));
+    if ((rc = trajectory(w)) < 0) return rc;
+    MhArgs m{};
+    m.D = D; m.N = N; m.n_steps = a.n_steps;
+    m.th0 = a.th_in; m.g0 = a.g_in; m.lp0 = a.lp_in; m.ld0 = a.ld_in;
+    m.r0 = w.r0; m.lk0 = w.lk0;
+    m.th = a.th_out; m.r = a.r_out; m.g = a.g_out; m.lp = a.lp_out; m.lk = a.lk_out; m.ld = a.ld_out;
+    m.rng = h.rng; m.st = h.st;
+    CU(launch_mh_select(m, ctx->stream, nl));
+    return AHMC_OK;
 }
 }  // namespace
 
@@ -489,13 +566,8 @@ int ahmc_destroy(ahmc_ctx* ctx) {
     DeviceGuard g(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     cudaFree(ctx->d_min_break);
-    cudaFree(ctx->arena);
-    cudaFree(ctx->nuts_scratch);
-    cudaFree(ctx->adapt_scratch);
-    cudaFree(ctx->mn_scratch);
-    cudaFree(ctx->dense_scratch);
-    cudaFree(ctx->coop_scratch);
-    cudaFree(ctx->split_scratch);
+    for (DevBuf* b : {&ctx->arena, &ctx->chain_ws, &ctx->summary_ws, &ctx->energy_ws, &ctx->dense_ws, &ctx->coop_ws, &ctx->split_ws})
+        cudaFree(b->p);
     for (int i = 0; i < ahmc_ctx::kPipeStreams; ++i) {
         if (ctx->pipe[i]) cudaStreamDestroy(ctx->pipe[i]);
         if (ctx->ev_join[i]) cudaEventDestroy(ctx->ev_join[i]);
@@ -664,23 +736,22 @@ int ahmc_phasepoint_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metri
     if (N == 0) return AHMC_OK;
     DeviceGuard g(ctx->device);
     Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
-    const size_t DN = (size_t)z->ld * N * sizeof(double), Nb = (size_t)N * sizeof(double);
-    reserve_metric(st, metric, D, N);
-    st.reserve(DN * 4);
-    st.reserve(Nb * 2);
-    if ((rc = st.prepare())) return rc;
     PhasepointArgs a{};
     a.model = model_dev(model);
-    if ((rc = stage_metric(st, metric, D, N, &a.metric))) return rc;
     a.D = D;
     a.N = N;
     a.ld = z->ld;
-    if ((rc = st.in((const double*)z->theta, (size_t)z->ld * N, &a.th))) return rc;
-    if ((rc = st.in((const double*)z->r, (size_t)z->ld * N, &a.r))) return rc;
-    if ((rc = st.out(z->lp_value, (size_t)N, &a.lp))) return rc;
-    if ((rc = st.out(z->lp_gradient, (size_t)z->ld * N, &a.g))) return rc;
-    if ((rc = st.out(z->lk_value, (size_t)N, &a.lk))) return rc;
-    if ((rc = st.out(z->lk_gradient, (size_t)z->ld * N, &a.dr))) return rc;
+    rc = st.stage([&](Stager& s) {
+        const size_t c = (size_t)z->ld * N;
+        stage_metric(s, metric, D, N, &a.metric);
+        s.in((const double*)z->theta, c, &a.th);
+        s.in((const double*)z->r, c, &a.r);
+        s.out(z->lp_value, (size_t)N, &a.lp);
+        s.out(z->lp_gradient, c, &a.g);
+        s.out(z->lk_value, (size_t)N, &a.lk);
+        s.out(z->lk_gradient, c, &a.dr);
+    });
+    if (rc) return rc;
     int nl = 0;
     if (model->kind == AHMC_MODEL_CALLBACK) {  // user closure, then the metric half of phasepoint
         SplitWork w;
@@ -845,45 +916,33 @@ static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const
 
     // device staging for whatever is not addressed directly
     const int64_t ldi = z_in->ld, ldo = z_out->ld;
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
     const size_t nMinv = metric_minv_count(metric, D, N);
     const bool stage_in = up != UP_DIRECT, stage_out = !down_direct;
     const bool hasU = metric->kind == AHMC_METRIC_DENSE && metric->cholU;
-    size_t need = (per_chain_minv && !stage_in ? 0 : al(nMinv * 8)) + (hasU ? al((size_t)D * D * 8) : 0);
-    if (stage_in) need += al((size_t)N * 8) + (has_g ? 3 : 2) * al((size_t)ldi * N * 8);
-    if (stage_out) need += 4 * al((size_t)ldo * N * 8) + 2 * al((size_t)N * 8) + 2 * al((size_t)N * 4);
-    if (need > ctx->arena_bytes) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        for (int i = 0; i < ahmc_ctx::kPipeStreams; ++i) CU(cudaStreamSynchronize(ctx->pipe[i]));
-        cudaFree(ctx->arena);
-        ctx->arena = nullptr;
-        ctx->arena_bytes = 0;
-        size_t cap = need + need / 4;
-        if (cudaMalloc((void**)&ctx->arena, cap) != cudaSuccess)
-            return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for staging failed", cap);
-        ctx->arena_bytes = cap;
-    }
-    size_t off = 0;
-    auto carve = [&](bool want, size_t bytes) -> char* {
-        if (!want || !bytes) return nullptr;
-        char* p = ctx->arena + off;
-        off += al(bytes);
-        return p;
+    double *dMinv, *dU, *dEps, *dTh, *dR, *dG, *oTh, *oR, *oG, *oDr, *oLp, *oLk;
+    uint32_t* oSt;
+    int32_t* oSd;
+    auto layout = [&](Carver& c) {
+        dMinv = c.take<double>(nMinv, nMinv && !(per_chain_minv && !stage_in));
+        dU = c.take<double>((size_t)D * D, hasU);
+        dEps = c.take<double>((size_t)N, stage_in);
+        dTh = c.take<double>((size_t)ldi * N, stage_in);
+        dR = c.take<double>((size_t)ldi * N, stage_in);
+        dG = c.take<double>((size_t)ldi * N, stage_in && has_g);
+        oTh = c.take<double>((size_t)ldo * N, stage_out);
+        oR = c.take<double>((size_t)ldo * N, stage_out);
+        oG = c.take<double>((size_t)ldo * N, stage_out);
+        oDr = c.take<double>((size_t)ldo * N, stage_out);
+        oLp = c.take<double>((size_t)N, stage_out);
+        oLk = c.take<double>((size_t)N, stage_out);
+        oSt = c.take<uint32_t>((size_t)N, stage_out);
+        oSd = c.take<int32_t>((size_t)N, stage_out);
     };
-    double* dMinv = (double*)carve(!(per_chain_minv && !stage_in), nMinv * 8);
-    double* dU = (double*)carve(hasU, (size_t)D * D * 8);
-    double* dEps = (double*)carve(stage_in, (size_t)N * 8);
-    double* dTh = (double*)carve(stage_in, (size_t)ldi * N * 8);
-    double* dR = (double*)carve(stage_in, (size_t)ldi * N * 8);
-    double* dG = (double*)carve(stage_in && has_g, (size_t)ldi * N * 8);
-    double* oTh = (double*)carve(stage_out, (size_t)ldo * N * 8);
-    double* oR = (double*)carve(stage_out, (size_t)ldo * N * 8);
-    double* oG = (double*)carve(stage_out, (size_t)ldo * N * 8);
-    double* oDr = (double*)carve(stage_out, (size_t)ldo * N * 8);
-    double* oLp = (double*)carve(stage_out, (size_t)N * 8);
-    double* oLk = (double*)carve(stage_out, (size_t)N * 8);
-    uint32_t* oSt = (uint32_t*)carve(stage_out, (size_t)N * 4);
-    int32_t* oSd = (int32_t*)carve(stage_out, (size_t)N * 4);
+    Carver size;
+    layout(size);
+    if ((rc = ensure_arena(ctx, size.off))) return rc;
+    Carver arena{(char*)ctx->arena.p};
+    layout(arena);
 
     cudaStream_t s_cmp = ctx->stream;
     cudaStream_t s_up[3] = {ctx->pipe[0], up == UP_CE3 ? ctx->pipe[1] : ctx->pipe[0], up == UP_CE3 ? ctx->pipe[2] : ctx->pipe[0]};
@@ -1070,37 +1129,25 @@ int ahmc_leapfrog_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric*
         return leapfrog_host_pipelined(ctx, model, metric, D, N, eps, eps_chain, n_steps, temper_alpha, z_in, z_out,
                                        status, steps_done, flags);
     Stager st(ctx, host);
-    const size_t cin = (size_t)z_in->ld * N, cout = (size_t)z_out->ld * N;
-    reserve_metric(st, metric, D, N);
-    st.reserve(cin * 8 * 3);
-    st.reserve(cout * 8 * 4);
-    st.reserve((size_t)N * 8 * 6);
-    if ((rc = st.prepare())) return rc;
     LeapfrogArgs a{};
     a.model = model_dev(model);
-    if ((rc = stage_metric(st, metric, D, N, &a.metric))) return rc;
     a.D = D;
     a.N = N;
     a.eps = eps;
-    if ((rc = st.in(eps_chain, (size_t)N, &a.eps_chain))) return rc;
     a.n_steps = n_abs;
     a.fwd = n_steps > 0;
     a.temper_alpha = temper_alpha;
-    a.ld_in = z_in->ld;
-    a.ld_out = z_out->ld;
-    if ((rc = st.in((const double*)z_in->theta, cin, &a.th_in))) return rc;
-    if ((rc = st.in((const double*)z_in->r, cin, &a.r_in))) return rc;
-    if ((rc = st.in((const double*)z_in->lp_gradient, cin, &a.g_in))) return rc;
     a.lp_in = nullptr;
     a.lk_in = nullptr;
-    if ((rc = st.out(z_out->theta, cout, &a.th_out))) return rc;
-    if ((rc = st.out(z_out->r, cout, &a.r_out))) return rc;
-    if ((rc = st.out(z_out->lp_gradient, cout, &a.g_out))) return rc;
-    if ((rc = st.out(z_out->lk_gradient, cout, &a.dr_out))) return rc;
-    if ((rc = st.out(z_out->lp_value, (size_t)N, &a.lp_out))) return rc;
-    if ((rc = st.out(z_out->lk_value, (size_t)N, &a.lk_out))) return rc;
-    if ((rc = st.out(status, (size_t)N, &a.status))) return rc;
-    if ((rc = st.out(steps_done, (size_t)N, &a.steps_done))) return rc;
+    rc = st.stage([&](Stager& s) {
+        stage_metric(s, metric, D, N, &a.metric);
+        s.in(eps_chain, (size_t)N, &a.eps_chain);
+        stage_pp_in(s, z_in, N, a);
+        stage_pp_out(s, z_out, (size_t)z_out->ld * N, (size_t)N, a, &a.dr_out);
+        s.out(status, (size_t)N, &a.status);
+        s.out(steps_done, (size_t)N, &a.steps_done);
+    });
+    if (rc) return rc;
     a.flags = flags;
     const bool compat = flags & AHMC_FLAG_COMPAT_BREAK_ALL;
     a.min_break = nullptr;
@@ -1174,19 +1221,18 @@ int ahmc_rand_momentum_f64(ahmc_ctx* ctx, const ahmc_metric* metric, int32_t D, 
     if (N == 0) return AHMC_OK;
     DeviceGuard g(ctx->device);
     Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
-    reserve_metric(st, metric, D, N);
-    st.reserve((size_t)D * N * 8);
-    st.reserve((size_t)ld * N * 8);
-    if ((rc = st.prepare())) return rc;
     MomentumArgs a{};
-    if ((rc = stage_metric(st, metric, D, N, &a.metric))) return rc;
     a.D = D;
     a.N = N;
     a.seed = rng->seed;
     a.offset = rng->offset;
-    if ((rc = st.in(rng->normal_tape, (size_t)D * N, &a.normal_tape))) return rc;
-    if ((rc = st.out(r, (size_t)ld * N, &a.r))) return rc;
     a.ld = ld;
+    rc = st.stage([&](Stager& s) {
+        stage_metric(s, metric, D, N, &a.metric);
+        s.in(rng->normal_tape, (size_t)D * N, &a.normal_tape);
+        s.out(r, (size_t)ld * N, &a.r);
+    });
+    if (rc) return rc;
     int nl = 0;
     CU(launch_rand_momentum(a, ctx->stream, &nl));
     ctx->launches += nl;
@@ -1194,33 +1240,46 @@ int ahmc_rand_momentum_f64(ahmc_ctx* ctx, const ahmc_metric* metric, int32_t D, 
 }
 
 // ---------------------------------------------------------------------------------------------- transitions
-static int stage_stats(Stager& st, const ahmc_stats* s, int64_t N, StatsDev* d) {
+static void stage_stats(Stager& st, const ahmc_stats* s, int64_t N, StatsDev* d) {
     memset(d, 0, sizeof *d);
-    if (!s) return AHMC_OK;
-    int rc;
-    if ((rc = st.out(s->n_steps, (size_t)N, &d->n_steps))) return rc;
-    if ((rc = st.out(s->is_accept, (size_t)N, &d->is_accept))) return rc;
-    if ((rc = st.out(s->acceptance_rate, (size_t)N, &d->acceptance_rate))) return rc;
-    if ((rc = st.out(s->log_density, (size_t)N, &d->log_density))) return rc;
-    if ((rc = st.out(s->hamiltonian_energy, (size_t)N, &d->hamiltonian_energy))) return rc;
-    if ((rc = st.out(s->hamiltonian_energy_error, (size_t)N, &d->hamiltonian_energy_error))) return rc;
-    if ((rc = st.out(s->max_hamiltonian_energy_error, (size_t)N, &d->max_hamiltonian_energy_error))) return rc;
-    if ((rc = st.out(s->tree_depth, (size_t)N, &d->tree_depth))) return rc;
-    if ((rc = st.out(s->numerical_error, (size_t)N, &d->numerical_error))) return rc;
-    return AHMC_OK;
+    if (!s) return;
+    st.out(s->n_steps, (size_t)N, &d->n_steps);
+    st.out(s->is_accept, (size_t)N, &d->is_accept);
+    st.out(s->acceptance_rate, (size_t)N, &d->acceptance_rate);
+    st.out(s->log_density, (size_t)N, &d->log_density);
+    st.out(s->hamiltonian_energy, (size_t)N, &d->hamiltonian_energy);
+    st.out(s->hamiltonian_energy_error, (size_t)N, &d->hamiltonian_energy_error);
+    st.out(s->max_hamiltonian_energy_error, (size_t)N, &d->max_hamiltonian_energy_error);
+    st.out(s->tree_depth, (size_t)N, &d->tree_depth);
+    st.out(s->numerical_error, (size_t)N, &d->numerical_error);
 }
 
-static int stage_rng(Stager& st, const ahmc_rng* r, int32_t D, int64_t N, bool nuts, RngDev* d) {
+static void stage_rng(Stager& st, const ahmc_rng* r, int32_t D, int64_t N, bool nuts, RngDev* d) {
     d->seed = r->seed;
     d->offset = r->offset;
     d->partial_alpha = r->partial_refresh_alpha;
     d->temper_alpha = r->temper_alpha > 0.0 ? r->temper_alpha : 0.0;
     d->exp_stride = nuts ? r->exp_stride : 1;
     d->dir_stride = r->dir_stride;
-    int rc;
-    if ((rc = st.in(r->normal_tape, (size_t)D * N, &d->normal_tape))) return rc;
-    if ((rc = st.in(r->exp_tape, (size_t)(nuts ? r->exp_stride : 1) * N, &d->exp_tape))) return rc;
-    if ((rc = st.in(nuts ? r->dir_tape : (const uint8_t*)nullptr, (size_t)r->dir_stride * N, &d->dir_tape))) return rc;
+    st.in(r->normal_tape, (size_t)D * N, &d->normal_tape);
+    st.in(r->exp_tape, (size_t)(nuts ? r->exp_stride : 1) * N, &d->exp_tape);
+    st.in(nuts ? r->dir_tape : (const uint8_t*)nullptr, (size_t)r->dir_stride * N, &d->dir_tape);
+}
+
+// the momentum refresh (partial_refresh_alpha) and integrator (temper_alpha) a transition's rng asks for
+static int check_refresh_rng(ahmc_ctx* ctx, const ahmc_rng* rng) {
+    if (!(rng->partial_refresh_alpha > -1.0 && rng->partial_refresh_alpha < 1.0))
+        return fail(ctx, AHMC_ERR_INVALID, "partial_refresh_alpha must be in (-1, 1)");
+    if (!(rng->temper_alpha >= 0.0) || std::isinf(rng->temper_alpha))
+        return fail(ctx, AHMC_ERR_INVALID, "temper_alpha must be 0 (plain Leapfrog) or a finite alpha > 0 (TemperedLeapfrog)");
+    return AHMC_OK;
+}
+// what every transition needs of its metric and output phase point
+static int check_transition_io(ahmc_ctx* ctx, const ahmc_metric* metric, const ahmc_phasepoint* z_out, uint32_t flags) {
+    if (metric->kind == AHMC_METRIC_DENSE && !metric->cholU && !(flags & AHMC_FLAG_NO_REFRESH))
+        return fail(ctx, AHMC_ERR_INVALID, "Dense metric needs cholU for the momentum refresh (metric.jl:311-320)");
+    if (z_out->lk_gradient)
+        return fail(ctx, AHMC_ERR_UNSUPPORTED, "transition entry points do not emit lk_gradient; call ahmc_phasepoint_f64 if needed");
     return AHMC_OK;
 }
 
@@ -1268,23 +1327,17 @@ static int check_adapt_cfg(ahmc_ctx* ctx, const ahmc_adapt_cfg* cfg, const ahmc_
         return fail(ctx, AHMC_ERR_INVALID, "need gamma > 0, t0 >= 0, 0 < delta < 1");
     return AHMC_OK;
 }
-// doubles of one chain's Minv_chain row: D, or D x D for a Dense metric (its rows also need the cholU_chain row; with step
-// size only both are optional and, when given, receive the starting metric)
-static size_t adapt_row_doubles(const ahmc_metric* metric, int32_t D) {
-    return metric->kind == AHMC_METRIC_DENSE ? (size_t)D * D : (size_t)D;
+// in-launch adaptation: the metric / estimator pair, then `refusal` (why this sampler configuration cannot adapt inside
+// its launch, or nullptr), then the cfg
+static int check_adapt(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, const ahmc_adapt_cfg* cfg,
+                       const ahmc_rng* rng, int32_t n_transitions, const char* refusal) {
+    int rc = check_adapt_metric(ctx, model, metric, cfg);
+    if (rc) return rc;
+    if (refusal) return fail(ctx, AHMC_ERR_UNSUPPORTED, "%s", refusal);
+    return check_adapt_cfg(ctx, cfg, rng, n_transitions);
 }
-static bool dense_rows(const ahmc_metric* metric, const ahmc_adapt_cfg* cfg) {
-    return metric->kind == AHMC_METRIC_DENSE && cfg->Minv_chain && cfg->cholU_chain;
-}
-static void reserve_adapt(Stager& st, const ahmc_metric* metric, const ahmc_adapt_cfg* cfg, int32_t D, int64_t N, int32_t n_transitions) {
-    st.reserve((size_t)N * 8);
-    if (cfg->Minv_chain) st.reserve((size_t)N * adapt_row_doubles(metric, D) * 8);
-    if (dense_rows(metric, cfg)) st.reserve((size_t)N * D * D * 8);
-    if (cfg->eps_trace) st.reserve((size_t)N * n_transitions * 8);
-}
-// fills `ad` (schedule, constants, staged eps / M^-1 / trace buffers); *eps_chain = the per-chain step sizes the kernel reads
-static int stage_adapt(ahmc_ctx* ctx, Stager& st, const ahmc_metric* metric, const ahmc_adapt_cfg* cfg, int32_t D, int64_t N,
-                       int32_t n_transitions, AdaptDev* ad, const double** eps_chain) {
+// fills `ad` with the schedule and constants of the adaptors
+static int adapt_schedule(ahmc_ctx* ctx, const ahmc_adapt_cfg* cfg, AdaptDev* ad) {
     ad->enabled = 1;
     ad->n_adapts = cfg->n_adapts;
     ad->delta = cfg->delta;
@@ -1296,34 +1349,40 @@ static int stage_adapt(ahmc_ctx* ctx, Stager& st, const ahmc_metric* metric, con
     if (!stan_window_schedule(*ad, cfg->init_buffer, cfg->term_buffer, cfg->window_size, cfg->n_adapts))
         return fail(ctx, AHMC_ERR_UNSUPPORTED, "the window schedule (stan_adaptor.jl:13-50) needs more than %d splits",
                     (int)(sizeof(ad->splits) / sizeof(ad->splits[0])));
-    int rc;
-    if ((rc = st.inout(cfg->eps_chain, (size_t)N, &ad->eps))) return rc;
-    *eps_chain = ad->eps;
-    if (metric->kind == AHMC_METRIC_DENSE) {  // the chain's M^-1 / factor rows: both or neither (step size only)
-        ad->minv = ad->cholU = nullptr;
-        if (dense_rows(metric, cfg)) {
-            if ((rc = st.out(cfg->Minv_chain, (size_t)N * D * D, &ad->minv))) return rc;
-            if ((rc = st.out(cfg->cholU_chain, (size_t)N * D * D, &ad->cholU))) return rc;
-        }
-    } else {
-        ad->cholU = nullptr;
-        if ((rc = st.out(cfg->Minv_chain, (size_t)N * D, &ad->minv))) return rc;
-    }
-    if ((rc = st.out(cfg->eps_trace, (size_t)N * n_transitions, &ad->eps_trace))) return rc;
     return AHMC_OK;
 }
-// the context's per-chain workspace (NUTS trees, in-launch adaptors' estimators): at least `need` bytes
-static int chain_workspace(ahmc_ctx* ctx, size_t need, double** out) {
-    if (need > ctx->nuts_scratch_bytes) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->nuts_scratch);
-        ctx->nuts_scratch = nullptr;
-        ctx->nuts_scratch_bytes = 0;
-        cudaError_t e = cudaMalloc((void**)&ctx->nuts_scratch, need);
-        if (e != cudaSuccess) return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for the NUTS workspace failed: %s", need, cudaGetErrorString(e));
-        ctx->nuts_scratch_bytes = need;
+// stages the adaptors' eps / M^-1 / trace buffers into `ad`; *eps_chain = the per-chain step sizes the kernel reads
+static void stage_adapt(Stager& st, const ahmc_metric* metric, const ahmc_adapt_cfg* cfg, int32_t D, int64_t N,
+                        int32_t n_transitions, AdaptDev* ad, const double** eps_chain) {
+    st.inout(cfg->eps_chain, (size_t)N, &ad->eps);
+    *eps_chain = ad->eps;
+    ad->minv = ad->cholU = nullptr;
+    if (metric->kind == AHMC_METRIC_DENSE) {  // the chain's M^-1 / factor rows: both or neither (step size only)
+        if (cfg->Minv_chain && cfg->cholU_chain) {
+            st.out(cfg->Minv_chain, (size_t)N * D * D, &ad->minv);
+            st.out(cfg->cholU_chain, (size_t)N * D * D, &ad->cholU);
+        }
+    } else {
+        st.out(cfg->Minv_chain, (size_t)N * D, &ad->minv);
     }
-    *out = ctx->nuts_scratch;
+    st.out(cfg->eps_trace, (size_t)N * n_transitions, &ad->eps_trace);
+}
+// the context's per-chain workspace (NUTS trees, in-launch adaptors' estimators, D > 512 start points): at least `need` bytes
+static int chain_workspace(ahmc_ctx* ctx, size_t need, double** out) {
+    int rc = ensure(ctx, ctx->chain_ws, need, "the NUTS workspace");
+    *out = (double*)ctx->chain_ws.p;
+    return rc;
+}
+// adapt_summary's workspace (K5): [completion counter (as 2 doubles)] [block partials], for `blocks` blocks.  The counter
+// starts at zero and the kernel leaves it at zero, so it is cleared only when the buffer is new.
+static int summary_workspace(ahmc_ctx* ctx, int32_t D, int blocks, unsigned** counter, double** partial) {
+    const size_t need = ((size_t)blocks * (D + 1) + 2) * sizeof(double);
+    const bool grows = need > ctx->summary_ws.bytes;
+    int rc = ensure(ctx, ctx->summary_ws, need, "the adaptor workspace");
+    if (rc) return rc;
+    if (grows) CU(cudaMemsetAsync(ctx->summary_ws.p, 0, need, ctx->stream));
+    *counter = (unsigned*)ctx->summary_ws.p;
+    *partial = (double*)ctx->summary_ws.p + 2;
     return AHMC_OK;
 }
 
@@ -1333,25 +1392,21 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
                     uint32_t flags, const ahmc_adapt_cfg* cfg = nullptr) {
     if (!ctx || !model || !metric || !rng) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/model/metric/rng");
     if (n_transitions < 1) return fail(ctx, AHMC_ERR_INVALID, "n_transitions must be >= 1");
-    if (cfg) {
-        int rc = check_adapt_metric(ctx, model, metric, cfg);
-        if (rc) return rc;
-        if (model->kind == AHMC_MODEL_CALLBACK)
-            return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation needs a device-resident target: callback (split-step) models cannot run inside one launch; express the target as CUDA source (ahmc_model_create_user)");
-        rc = check_adapt_cfg(ctx, cfg, rng, n_transitions);
-        if (rc) return rc;
-    }
+    int rc;
+    if (cfg &&
+        (rc = check_adapt(ctx, model, metric, cfg, rng, n_transitions,
+                          model->kind == AHMC_MODEL_CALLBACK
+                              ? "in-launch adaptation needs a device-resident target: callback (split-step) models cannot run inside one launch; express the target as CUDA source (ahmc_model_create_user)"
+                              : nullptr)))
+        return rc;
     if (n_transitions > 1 && (rng->normal_tape || rng->exp_tape))
         return fail(ctx, AHMC_ERR_INVALID, "random tapes describe ONE transition; multi-transition sampling uses the Philox streams");
     if (n_transitions > 1 && model->kind == AHMC_MODEL_CALLBACK)
         return fail(ctx, AHMC_ERR_UNSUPPORTED, "multi-transition sampling needs a device-resident target");
     if (rng->partial_refresh_alpha != 0.0 && model->kind == AHMC_MODEL_CALLBACK)
         return fail(ctx, AHMC_ERR_UNSUPPORTED, "partial momentum refreshment is not wired into the split-step path");
-    if (!(rng->partial_refresh_alpha > -1.0 && rng->partial_refresh_alpha < 1.0))
-        return fail(ctx, AHMC_ERR_INVALID, "partial_refresh_alpha must be in (-1, 1)");
-    if (!(rng->temper_alpha >= 0.0) || std::isinf(rng->temper_alpha))
-        return fail(ctx, AHMC_ERR_INVALID, "temper_alpha must be 0 (plain Leapfrog) or a finite alpha > 0 (TemperedLeapfrog)");
-    int rc = check_common(ctx, model, metric, D, N, true);
+    if ((rc = check_refresh_rng(ctx, rng))) return rc;
+    rc = check_common(ctx, model, metric, D, N, true);
     if (!rc && D > 512 && rng->temper_alpha > 0.0) rc = fail(ctx, AHMC_ERR_UNSUPPORTED, "TemperedLeapfrog at D > 512 is not built");
     if (!rc && D > 512 && !(flags & AHMC_FLAG_NO_REFRESH) && !rng->normal_tape) rc = check_philox_d(ctx, D);
     if (rc) return rc;
@@ -1360,143 +1415,57 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
     if (n_steps < 1) return fail(ctx, AHMC_ERR_INVALID, "n_steps must be >= 1 (nsteps(tau) = max(1, ...), trajectory.jl:240-243)");
     if (flags & AHMC_FLAG_COMPAT_BREAK_ALL)
         return fail(ctx, AHMC_ERR_UNSUPPORTED, "COMPAT_BREAK_ALL is only available on ahmc_leapfrog_f64");
-    if (metric->kind == AHMC_METRIC_DENSE && !metric->cholU && !(flags & AHMC_FLAG_NO_REFRESH))
-        return fail(ctx, AHMC_ERR_INVALID, "Dense metric needs cholU for the momentum refresh (metric.jl:311-320)");
-    if (z_out->lk_gradient)
-        return fail(ctx, AHMC_ERR_UNSUPPORTED, "transition entry points do not emit lk_gradient; call ahmc_phasepoint_f64 if needed");
+    if ((rc = check_transition_io(ctx, metric, z_out, flags))) return rc;
     if (N == 0) return AHMC_OK;
+    HmcArgs h{};
+    if (cfg && (rc = adapt_schedule(ctx, cfg, &h.ad))) return rc;
     DeviceGuard g(ctx->device);
     Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
-    const size_t cin = (size_t)z_in->ld * N, cout = (size_t)z_out->ld * N;
-    reserve_metric(st, metric, D, N);
-    st.reserve(cin * 8 * 3);
-    st.reserve(cout * 8 * 3);
-    st.reserve((size_t)D * N * 8);
-    st.reserve((size_t)N * 8 * 16 * n_transitions);
-    if (draws) st.reserve((size_t)D * N * n_transitions * 8);
-    if (cfg) reserve_adapt(st, metric, cfg, D, N, n_transitions);
-    if ((rc = st.prepare())) return rc;
-    HmcArgs h{};
     LeapfrogArgs& a = h.lf;
     a.model = model_dev(model);
-    if ((rc = stage_metric(st, metric, D, N, &a.metric))) return rc;
     a.D = D;
     a.N = N;
     a.eps = eps;
-    if (cfg) {
-        if ((rc = stage_adapt(ctx, st, metric, cfg, D, N, n_transitions, &h.ad, &a.eps_chain))) return rc;
-    } else if ((rc = st.in(eps_chain, (size_t)N, &a.eps_chain))) {
-        return rc;
-    }
     a.n_steps = n_steps;
     a.fwd = 1;
     a.temper_alpha = 0.0;
-    a.ld_in = z_in->ld;
-    a.ld_out = z_out->ld;
-    if ((rc = st.in((const double*)z_in->theta, cin, &a.th_in))) return rc;
-    if ((rc = st.in((const double*)z_in->r, cin, &a.r_in))) return rc;
-    if ((rc = st.in((const double*)z_in->lp_gradient, cin, &a.g_in))) return rc;
-    if ((rc = st.in((const double*)z_in->lp_value, (size_t)N, &a.lp_in))) return rc;
-    if ((rc = st.out(z_out->theta, cout, &a.th_out))) return rc;
-    if ((rc = st.out(z_out->r, cout, &a.r_out))) return rc;
-    if ((rc = st.out(z_out->lp_gradient, cout, &a.g_out))) return rc;
-    if ((rc = st.out(z_out->lp_value, (size_t)N, &a.lp_out))) return rc;
-    if ((rc = st.out(z_out->lk_value, (size_t)N, &a.lk_out))) return rc;
     a.dr_out = nullptr;
     a.flags = flags;
-    if ((rc = stage_rng(st, rng, D, N, false, &h.rng))) return rc;
-    if ((rc = stage_stats(st, stats, N * n_transitions, &h.st))) return rc;
-    if ((rc = st.out(draws, (size_t)D * N * n_transitions, &h.draws))) return rc;
     h.n_transitions = n_transitions;
     h.refresh = (flags & AHMC_FLAG_NO_REFRESH) ? 0 : 1;
+    rc = st.stage([&](Stager& s) {
+        stage_metric(s, metric, D, N, &a.metric);
+        if (cfg) stage_adapt(s, metric, cfg, D, N, n_transitions, &h.ad, &a.eps_chain);
+        else s.in(eps_chain, (size_t)N, &a.eps_chain);
+        stage_pp_in(s, z_in, N, a, &a.lp_in);
+        stage_pp_out(s, z_out, (size_t)z_out->ld * N, (size_t)N, a);
+        stage_rng(s, rng, D, N, false, &h.rng);
+        stage_stats(s, stats, N * n_transitions, &h.st);
+        s.out(draws, (size_t)D * N * n_transitions, &h.draws);
+    });
+    if (rc) return rc;
     int nl = 0;
     if (model->kind == AHMC_MODEL_CALLBACK) {
-        // refresh -> kinetic energy -> split-step trajectory -> MH select (same semantics as hmc_kernel, unfused)
-        SplitWork w;
-        if ((rc = split_workspace(ctx, D, N, z_out->ld, &w))) return rc;
-        if (h.refresh) {
-            MomentumArgs ma{};
-            ma.metric = a.metric; ma.D = D; ma.N = N; ma.seed = h.rng.seed; ma.offset = h.rng.offset;
-            ma.normal_tape = h.rng.normal_tape; ma.r = w.r0; ma.ld = D;
-            CU(launch_rand_momentum(ma, ctx->stream, &nl));
-        } else {
-            CU(cudaMemcpy2DAsync(w.r0, (size_t)D * 8, a.r_in, (size_t)a.ld_in * 8, (size_t)D * 8, (size_t)N,
-                                 cudaMemcpyDeviceToDevice, ctx->stream));
-        }
-        SplitArgs k0{};  // lk0 = neg kinetic energy of the refreshed momentum
-        k0.metric = a.metric; k0.D = D; k0.N = N; k0.fwd = 1; k0.mul = 1.0; k0.no_kick = 1;
-        k0.r = w.r0; k0.lk = w.lk0; k0.ld = D;
-        CU(launch_kick_energy(k0, ctx->stream, &nl));
-        auto cp = [&](double* dst, const double* src, int64_t lds) -> cudaError_t {
-            if (dst == src) return cudaSuccess;
-            return cudaMemcpy2DAsync(dst, (size_t)a.ld_out * 8, src, (size_t)lds * 8, (size_t)D * 8, (size_t)N,
-                                     cudaMemcpyDeviceToDevice, ctx->stream);
-        };
-        if (a.th_out == a.th_in)
-            return fail(ctx, AHMC_ERR_INVALID, "callback-mode transitions need z_out distinct from z_in (the start point is re-read on rejection)");
-        CU(cp(a.th_out, a.th_in, a.ld_in));
-        CU(cp(a.g_out, a.g_in, a.ld_in));
-        CU(cp(a.r_out, w.r0, D));
-        rc = split_trajectory(ctx, model, a.metric, D, N, eps, a.eps_chain, n_steps, 1, h.rng.temper_alpha, a.th_out, a.r_out, a.g_out,
-                              a.lp_out, a.lk_out, nullptr, a.ld_out, w.status, w.steps, w, false, &nl);
+        rc = unfused_transition(ctx, h, &nl, [&](const SplitWork& w) {
+            return split_trajectory(ctx, model, a.metric, D, N, eps, a.eps_chain, n_steps, 1, h.rng.temper_alpha, a.th_out, a.r_out,
+                                    a.g_out, a.lp_out, a.lk_out, nullptr, a.ld_out, w.status, w.steps, w, false, &nl);
+        });
         if (rc) return rc;
-        MhArgs m{};
-        m.D = D; m.N = N; m.n_steps = n_steps;
-        m.th0 = a.th_in; m.g0 = a.g_in; m.lp0 = a.lp_in; m.ld0 = a.ld_in;
-        m.r0 = w.r0; m.lk0 = w.lk0;
-        m.th = a.th_out; m.r = a.r_out; m.g = a.g_out; m.lp = a.lp_out; m.lk = a.lk_out; m.ld = a.ld_out;
-        m.rng = h.rng; m.st = h.st;
-        CU(launch_mh_select(m, ctx->stream, &nl));
         ctx->launches += nl;
         return finish_call(ctx, st, flags);
     }
     if (!cfg && n_transitions == 1 && a.th_out != a.th_in && h.rng.partial_alpha == 0.0 && !(h.rng.temper_alpha > 0.0) && !draws &&
-        (model->kind == AHMC_MODEL_DENSE_GAUSS || a.metric.kind == AHMC_METRIC_DENSE)) {
-        // GEMM-shaped operators: refresh -> tiled DMMA trajectory (in place on z_out) -> MH select; same semantics as
-        // hmc_kernel.  (Falls through to the fused generic kernel when the tile kernel is not eligible.)
-        SplitWork w;
-        if ((rc = split_workspace(ctx, D, N, z_out->ld, &w))) return rc;
-        LeapfrogArgs t = a;
-        t.th_in = a.th_out; t.r_in = a.r_out; t.g_in = a.g_out; t.ld_in = a.ld_out;
-        t.status = nullptr; t.steps_done = nullptr; t.only_mask = nullptr; t.min_break = nullptr;
-        const bool gauss = model->kind != AHMC_MODEL_FUNNEL && model->kind != AHMC_MODEL_CALLBACK && model->kind != AHMC_MODEL_USER;
-        const bool metric_ok = a.metric.chain_stride == 0;  // shared M^-1 (the tile kernel's chains share one matrix)
-        int Dp_, RB_, CB_;
-        if (gauss && metric_ok && !(flags & AHMC_FLAG_EXACT_CHECKS) && dense_tile_shape(D, &Dp_, &RB_, &CB_)) {
-            if (h.refresh) {
-                MomentumArgs ma{};
-                ma.metric = a.metric; ma.D = D; ma.N = N; ma.seed = h.rng.seed; ma.offset = h.rng.offset;
-                ma.normal_tape = h.rng.normal_tape; ma.r = w.r0; ma.ld = D;
-                CU(launch_rand_momentum(ma, ctx->stream, &nl));
-            } else {
-                CU(cudaMemcpy2DAsync(w.r0, (size_t)D * 8, a.r_in, (size_t)a.ld_in * 8, (size_t)D * 8, (size_t)N,
-                                     cudaMemcpyDeviceToDevice, ctx->stream));
-            }
-            SplitArgs k0{};
-            k0.metric = a.metric; k0.D = D; k0.N = N; k0.fwd = 1; k0.mul = 1.0; k0.no_kick = 1;
-            k0.r = w.r0; k0.lk = w.lk0; k0.ld = D;
-            CU(launch_kick_energy(k0, ctx->stream, &nl));
-            auto cp = [&](double* dst, const double* src, int64_t lds) -> cudaError_t {
-                return cudaMemcpy2DAsync(dst, (size_t)a.ld_out * 8, src, (size_t)lds * 8, (size_t)D * 8, (size_t)N,
-                                         cudaMemcpyDeviceToDevice, ctx->stream);
-            };
-            CU(cp(a.th_out, a.th_in, a.ld_in));
-            CU(cp(a.g_out, a.g_in, a.ld_in));
-            CU(cp(a.r_out, w.r0, D));
-            rc = try_dense_trajectory(ctx, model, t, n_steps, eps, 0.0, false, &nl);
-            if (rc < 0) return rc;
-            if (rc == 1) {
-                MhArgs m{};
-                m.D = D; m.N = N; m.n_steps = n_steps;
-                m.th0 = a.th_in; m.g0 = a.g_in; m.lp0 = a.lp_in; m.ld0 = a.ld_in;
-                m.r0 = w.r0; m.lk0 = w.lk0;
-                m.th = a.th_out; m.r = a.r_out; m.g = a.g_out; m.lp = a.lp_out; m.lk = a.lk_out; m.ld = a.ld_out;
-                m.rng = h.rng; m.st = h.st;
-                CU(launch_mh_select(m, ctx->stream, &nl));
-                ctx->launches += nl;
-                return finish_call(ctx, st, flags);
-            }
-        }
+        dense_tile_eligible(model, a.metric, flags, D)) {
+        // GEMM-shaped operators: the tiled DMMA trajectory, in place on z_out
+        rc = unfused_transition(ctx, h, &nl, [&](const SplitWork&) {
+            LeapfrogArgs t = a;
+            t.th_in = a.th_out; t.r_in = a.r_out; t.g_in = a.g_out; t.ld_in = a.ld_out;
+            t.status = nullptr; t.steps_done = nullptr; t.only_mask = nullptr; t.min_break = nullptr;
+            return try_dense_trajectory(ctx, model, t, n_steps, eps, 0.0, false, &nl);
+        });
+        if (rc) return rc;
+        ctx->launches += nl;
+        return finish_call(ctx, st, flags);
     }
     if (cfg || D > 512) {  // the adaptors' estimator state: chain_adapt_doubles per chain; at D > 512 also the
                            // transition's start point, kBigHmcVectors D-vectors per chain ahead of it (ahmc_bigd_hmc.cu)
@@ -1514,22 +1483,16 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
                      const ahmc_stats* stats, uint32_t flags, const ahmc_adapt_cfg* cfg = nullptr) {
     if (!ctx || !model || !metric || !rng) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/model/metric/rng");
     if (n_transitions < 1) return fail(ctx, AHMC_ERR_INVALID, "n_transitions must be >= 1");
-    if (cfg) {
-        int rc = check_adapt_metric(ctx, model, metric, cfg);
-        if (rc) return rc;
-        if (flags & (AHMC_FLAG_NUTS_SLICE_TS | AHMC_FLAG_NUTS_CLASSIC | AHMC_FLAG_NUTS_STRICT))
-            return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation is built for MultinomialTS + GeneralisedNoUTurn");
-        rc = check_adapt_cfg(ctx, cfg, rng, n_transitions);
-        if (rc) return rc;
-    }
+    int rc;
+    if (cfg && (rc = check_adapt(ctx, model, metric, cfg, rng, n_transitions,
+                                 (flags & (AHMC_FLAG_NUTS_SLICE_TS | AHMC_FLAG_NUTS_CLASSIC | AHMC_FLAG_NUTS_STRICT))
+                                     ? "in-launch adaptation is built for MultinomialTS + GeneralisedNoUTurn"
+                                     : nullptr)))
+        return rc;
     if (n_transitions > 1 && (rng->normal_tape || rng->exp_tape || rng->dir_tape))
         return fail(ctx, AHMC_ERR_INVALID, "random tapes describe ONE transition; multi-transition sampling uses the Philox streams");
-    if (!(rng->partial_refresh_alpha > -1.0 && rng->partial_refresh_alpha < 1.0))
-        return fail(ctx, AHMC_ERR_INVALID, "partial_refresh_alpha must be in (-1, 1)");
-    if (!(rng->temper_alpha >= 0.0) || std::isinf(rng->temper_alpha))
-        return fail(ctx, AHMC_ERR_INVALID, "temper_alpha must be 0 (plain Leapfrog) or a finite alpha > 0 (TemperedLeapfrog)");
-    int rc = check_common(ctx, model, metric, D, N);
-    if (rc) return rc;
+    if ((rc = check_refresh_rng(ctx, rng))) return rc;
+    if ((rc = check_common(ctx, model, metric, D, N))) return rc;
     if ((rc = check_pp(ctx, z_in, D, "z_in", true, N))) return rc;
     if ((rc = check_pp(ctx, z_out, D, "z_out", true, N))) return rc;
     if (max_depth < 0 || max_depth > 20) return fail(ctx, AHMC_ERR_INVALID, "max_depth must be in 0..20");
@@ -1541,83 +1504,53 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
         return fail(ctx, AHMC_ERR_UNSUPPORTED, "NUTS needs a device-resident target: callback (split-step) models are supported by ahmc_leapfrog_f64 / ahmc_hmc_transition_f64 / ahmc_phasepoint_f64 only; express the target as CUDA source (ahmc_model_create_user) to run NUTS on it");
     if (model->kind == AHMC_MODEL_USER && (flags & (AHMC_FLAG_NUTS_SLICE_TS | AHMC_FLAG_NUTS_CLASSIC | AHMC_FLAG_NUTS_STRICT)))
         return fail(ctx, AHMC_ERR_UNSUPPORTED, "run-time compiled targets: MultinomialTS + GeneralisedNoUTurn only");
-    if (metric->kind == AHMC_METRIC_DENSE && !metric->cholU && !(flags & AHMC_FLAG_NO_REFRESH))
-        return fail(ctx, AHMC_ERR_INVALID, "Dense metric needs cholU for the momentum refresh (metric.jl:311-320)");
-    if (z_out->lk_gradient)
-        return fail(ctx, AHMC_ERR_UNSUPPORTED, "transition entry points do not emit lk_gradient; call ahmc_phasepoint_f64 if needed");
+    if ((rc = check_transition_io(ctx, metric, z_out, flags))) return rc;
     if (rng->exp_tape && rng->exp_stride < 1) return fail(ctx, AHMC_ERR_INVALID, "exp_tape needs exp_stride >= 1");
     if (rng->dir_tape && rng->dir_stride < max_depth) return fail(ctx, AHMC_ERR_INVALID, "dir_tape needs dir_stride >= max_depth");
     if (N == 0) return AHMC_OK;
+    NutsArgs a{};
+    if (cfg && (rc = adapt_schedule(ctx, cfg, &a.ad))) return rc;
     DeviceGuard g(ctx->device);
     Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
-    const size_t cin = (size_t)z_in->ld * N, cout = (size_t)z_out->ld * N;
-    reserve_metric(st, metric, D, N);
-    st.reserve(cin * 8 * 3);
-    st.reserve(cout * 8 * 3);
-    st.reserve((size_t)D * N * 8);
-    st.reserve((size_t)N * 8 * 16 * n_transitions);
-    if (draws) st.reserve((size_t)D * N * n_transitions * 8);
-    if (rng->exp_tape) st.reserve((size_t)rng->exp_stride * N * 8);
-    if (rng->dir_tape) st.reserve((size_t)rng->dir_stride * N);
-    if (cfg) reserve_adapt(st, metric, cfg, D, N, n_transitions);
-    if ((rc = st.prepare())) return rc;
-    NutsArgs a{};
     a.model = model_dev(model);
-    if ((rc = stage_metric(st, metric, D, N, &a.metric))) return rc;
-    int n_prep = 0;
-    if (a.metric.kind == AHMC_METRIC_DENSE && a.metric.chain_stride == 0 && !cfg && D > 16 && D <= 512) {
-        // the cooperative form streams Minv / cholU in chunks of columns: hand it copies whose columns are padded to the
-        // shared-memory leading dimension, so that a chunk is one bulk copy (two small kernels per call, on the stream).
-        // (A per-chain Dense metric, and the Dense adaptive form, run warp per chain: no shared matrix to pad.)
-        const size_t per = coop_padded_doubles(D);
-        if (2 * per > ctx->coop_scratch_doubles) {
-            CU(cudaStreamSynchronize(ctx->stream));
-            cudaFree(ctx->coop_scratch);
-            ctx->coop_scratch = nullptr;
-            ctx->coop_scratch_doubles = 0;
-            if (cudaMalloc((void**)&ctx->coop_scratch, 2 * per * sizeof(double)) != cudaSuccess)
-                return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc for the column-padded metric failed");
-            ctx->coop_scratch_doubles = 2 * per;
-        }
-        CU(launch_pad_columns(a.metric.Minv, D, ctx->coop_scratch, ctx->stream));
-        a.metric.Minv_coop = ctx->coop_scratch;
-        ++n_prep;
-        if (a.metric.cholU) {
-            CU(launch_pad_columns(a.metric.cholU, D, ctx->coop_scratch + per, ctx->stream));
-            a.metric.cholU_coop = ctx->coop_scratch + per;
-            ++n_prep;
-        }
-    }
-    ctx->launches += n_prep;
     a.D = D;
     a.N = N;
     a.eps = eps;
-    if (cfg) {
-        if ((rc = stage_adapt(ctx, st, metric, cfg, D, N, n_transitions, &a.ad, &a.eps_chain))) return rc;
-    } else if ((rc = st.in(eps_chain, (size_t)N, &a.eps_chain))) {
-        return rc;
-    }
     a.max_depth = max_depth;
     a.delta_max = delta_max;
     a.sampler = (flags & AHMC_FLAG_NUTS_SLICE_TS) ? 1 : 0;
     a.criterion = (flags & AHMC_FLAG_NUTS_STRICT) ? 2 : (flags & AHMC_FLAG_NUTS_CLASSIC) ? 1 : 0;
     a.refresh = (flags & AHMC_FLAG_NO_REFRESH) ? 0 : 1;
-    a.ld_in = z_in->ld;
-    a.ld_out = z_out->ld;
-    if ((rc = st.in((const double*)z_in->theta, cin, &a.th_in))) return rc;
-    if ((rc = st.in((const double*)z_in->r, cin, &a.r_in))) return rc;
-    if ((rc = st.in((const double*)z_in->lp_gradient, cin, &a.g_in))) return rc;
-    if ((rc = st.in((const double*)z_in->lp_value, (size_t)N, &a.lp_in))) return rc;
-    if ((rc = st.out(z_out->theta, cout, &a.th_out))) return rc;
-    if ((rc = st.out(z_out->r, cout, &a.r_out))) return rc;
-    if ((rc = st.out(z_out->lp_gradient, cout, &a.g_out))) return rc;
-    if ((rc = st.out(z_out->lp_value, (size_t)N, &a.lp_out))) return rc;
-    if ((rc = st.out(z_out->lk_value, (size_t)N, &a.lk_out))) return rc;
     a.dr_out = nullptr;
-    if ((rc = stage_rng(st, rng, D, N, true, &a.rng))) return rc;
-    if ((rc = stage_stats(st, stats, N * n_transitions, &a.st))) return rc;
-    if ((rc = st.out(draws, (size_t)D * N * n_transitions, &a.draws))) return rc;
     a.n_transitions = n_transitions;
+    rc = st.stage([&](Stager& s) {
+        stage_metric(s, metric, D, N, &a.metric);
+        if (cfg) stage_adapt(s, metric, cfg, D, N, n_transitions, &a.ad, &a.eps_chain);
+        else s.in(eps_chain, (size_t)N, &a.eps_chain);
+        stage_pp_in(s, z_in, N, a, &a.lp_in);
+        stage_pp_out(s, z_out, (size_t)z_out->ld * N, (size_t)N, a);
+        stage_rng(s, rng, D, N, true, &a.rng);
+        stage_stats(s, stats, N * n_transitions, &a.st);
+        s.out(draws, (size_t)D * N * n_transitions, &a.draws);
+    });
+    if (rc) return rc;
+    if (a.metric.kind == AHMC_METRIC_DENSE && a.metric.chain_stride == 0 && !cfg && D > 16 && D <= 512) {
+        // the cooperative form streams Minv / cholU in chunks of columns: hand it copies whose columns are padded to the
+        // shared-memory leading dimension, so that a chunk is one bulk copy (two small kernels per call, on the stream).
+        // (A per-chain Dense metric, and the Dense adaptive form, run warp per chain: no shared matrix to pad.)
+        const size_t per = coop_padded_doubles(D);
+        if ((rc = ensure(ctx, ctx->coop_ws, 2 * per * sizeof(double), "the column-padded metric"))) return rc;
+        double* coop = (double*)ctx->coop_ws.p;
+        CU(launch_pad_columns(a.metric.Minv, D, coop, ctx->stream));
+        a.metric.Minv_coop = coop;
+        int n_prep = 1;
+        if (a.metric.cholU) {
+            CU(launch_pad_columns(a.metric.cholU, D, coop + per, ctx->stream));
+            a.metric.cholU_coop = coop + per;
+            ++n_prep;
+        }
+        ctx->launches += n_prep;
+    }
     // per-chain tree workspace
     a.scratch_stride = nuts_scratch_doubles_per_chain(D, max_depth, cfg ? chain_adapt_doubles(cfg->adapt_metric, D) : 0);
     if ((rc = chain_workspace(ctx, (size_t)a.scratch_stride * (size_t)N * sizeof(double), &a.scratch))) return rc;
@@ -1643,29 +1576,19 @@ int ahmc_leapfrog_trajectory_f64(ahmc_ctx* ctx, const ahmc_model* model, const a
         return fail(ctx, AHMC_ERR_UNSUPPORTED, "full_trajectory: built-in targets only (callback / run-time compiled targets: loop over ahmc_leapfrog_f64)");
     DeviceGuard g(ctx->device);
     Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
-    const size_t cin = (size_t)z_in->ld * N, ctraj = (size_t)step_stride * n_abs;
-    reserve_metric(st, metric, D, N);
-    st.reserve(cin * 8 * 3);
-    st.reserve(ctraj * 8 * 4);
-    st.reserve((size_t)N * n_abs * 8 * 2 + (size_t)N * 16);
-    if ((rc = st.prepare())) return rc;
     TrajArgs a{};
     a.model = model_dev(model);
-    if ((rc = stage_metric(st, metric, D, N, &a.metric))) return rc;
     a.D = D; a.N = N; a.eps = eps;
-    if ((rc = st.in(eps_chain, (size_t)N, &a.eps_chain))) return rc;
     a.n_steps = n_abs; a.fwd = n_steps > 0; a.temper_alpha = temper_alpha;
-    a.ld_in = z_in->ld; a.ld_out = traj->ld; a.step_stride = step_stride;
-    if ((rc = st.in((const double*)z_in->theta, cin, &a.th_in))) return rc;
-    if ((rc = st.in((const double*)z_in->r, cin, &a.r_in))) return rc;
-    if ((rc = st.in((const double*)z_in->lp_gradient, cin, &a.g_in))) return rc;
-    if ((rc = st.out(traj->theta, ctraj, &a.th_out))) return rc;
-    if ((rc = st.out(traj->r, ctraj, &a.r_out))) return rc;
-    if ((rc = st.out(traj->lp_gradient, ctraj, &a.g_out))) return rc;
-    if ((rc = st.out(traj->lk_gradient, ctraj, &a.dr_out))) return rc;
-    if ((rc = st.out(traj->lp_value, (size_t)N * n_abs, &a.lp_out))) return rc;
-    if ((rc = st.out(traj->lk_value, (size_t)N * n_abs, &a.lk_out))) return rc;
-    if ((rc = st.out(steps_done, (size_t)N, &a.steps_done))) return rc;
+    a.step_stride = step_stride;
+    rc = st.stage([&](Stager& s) {
+        stage_metric(s, metric, D, N, &a.metric);
+        s.in(eps_chain, (size_t)N, &a.eps_chain);
+        stage_pp_in(s, z_in, N, a);
+        stage_pp_out(s, traj, (size_t)step_stride * n_abs, (size_t)N * n_abs, a, &a.dr_out);
+        s.out(steps_done, (size_t)N, &a.steps_done);
+    });
+    if (rc) return rc;
     int nl = 0;
     CU(launch_trajectory(a, ctx->stream, &nl));
     ctx->launches += nl;
@@ -1685,54 +1608,28 @@ int ahmc_hmc_multinomial_transition_f64(ahmc_ctx* ctx, const ahmc_model* model, 
         return fail(ctx, AHMC_ERR_INVALID, "need n_steps >= 1 and 0 <= n_steps_fwd <= n_steps (rand(0:n_steps), trajectory.jl:373)");
     if (model->kind == AHMC_MODEL_CALLBACK || model->kind == AHMC_MODEL_USER)
         return fail(ctx, AHMC_ERR_UNSUPPORTED, "MultinomialTS static transitions: built-in targets only");
-    if (metric->kind == AHMC_METRIC_DENSE && !metric->cholU && !(flags & AHMC_FLAG_NO_REFRESH))
-        return fail(ctx, AHMC_ERR_INVALID, "Dense metric needs cholU for the momentum refresh (metric.jl:311-320)");
-    if (z_out->lk_gradient)
-        return fail(ctx, AHMC_ERR_UNSUPPORTED, "transition entry points do not emit lk_gradient; call ahmc_phasepoint_f64 if needed");
-    if (!(rng->partial_refresh_alpha > -1.0 && rng->partial_refresh_alpha < 1.0))
-        return fail(ctx, AHMC_ERR_INVALID, "partial_refresh_alpha must be in (-1, 1)");
-    if (!(rng->temper_alpha >= 0.0) || std::isinf(rng->temper_alpha))
-        return fail(ctx, AHMC_ERR_INVALID, "temper_alpha must be 0 (plain Leapfrog) or a finite alpha > 0 (TemperedLeapfrog)");
+    if ((rc = check_transition_io(ctx, metric, z_out, flags))) return rc;
+    if ((rc = check_refresh_rng(ctx, rng))) return rc;
     if (N == 0) return AHMC_OK;
     DeviceGuard g(ctx->device);
     Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
-    const size_t cin = (size_t)z_in->ld * N, cout = (size_t)z_out->ld * N;
-    reserve_metric(st, metric, D, N);
-    st.reserve(cin * 8 * 3);
-    st.reserve(cout * 8 * 3);
-    st.reserve((size_t)D * N * 8);
-    st.reserve((size_t)N * 8 * 16);
-    if ((rc = st.prepare())) return rc;
     MultinomialArgs a{};
     a.model = model_dev(model);
-    if ((rc = stage_metric(st, metric, D, N, &a.metric))) return rc;
     a.D = D; a.N = N; a.eps = eps;
-    if ((rc = st.in(eps_chain, (size_t)N, &a.eps_chain))) return rc;
     a.n_steps = n_steps; a.n_fwd = n_steps_fwd;
     a.refresh = (flags & AHMC_FLAG_NO_REFRESH) ? 0 : 1;
-    a.ld_in = z_in->ld; a.ld_out = z_out->ld;
-    if ((rc = st.in((const double*)z_in->theta, cin, &a.th_in))) return rc;
-    if ((rc = st.in((const double*)z_in->r, cin, &a.r_in))) return rc;
-    if ((rc = st.in((const double*)z_in->lp_gradient, cin, &a.g_in))) return rc;
-    if ((rc = st.in((const double*)z_in->lp_value, (size_t)N, &a.lp_in))) return rc;
-    if ((rc = st.out(z_out->theta, cout, &a.th_out))) return rc;
-    if ((rc = st.out(z_out->r, cout, &a.r_out))) return rc;
-    if ((rc = st.out(z_out->lp_gradient, cout, &a.g_out))) return rc;
-    if ((rc = st.out(z_out->lp_value, (size_t)N, &a.lp_out))) return rc;
-    if ((rc = st.out(z_out->lk_value, (size_t)N, &a.lk_out))) return rc;
-    if ((rc = stage_rng(st, rng, D, N, false, &a.rng))) return rc;
-    if ((rc = stage_stats(st, stats, N, &a.st))) return rc;
-    const size_t need = (size_t)(n_steps + 1) * (size_t)N * sizeof(double);
-    if (need > ctx->mn_scratch_bytes) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->mn_scratch);
-        ctx->mn_scratch = nullptr;
-        ctx->mn_scratch_bytes = 0;
-        if (cudaMalloc((void**)&ctx->mn_scratch, need) != cudaSuccess)
-            return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for the multinomial energy tape failed", need);
-        ctx->mn_scratch_bytes = need;
-    }
-    a.energies = ctx->mn_scratch;
+    rc = st.stage([&](Stager& s) {
+        stage_metric(s, metric, D, N, &a.metric);
+        s.in(eps_chain, (size_t)N, &a.eps_chain);
+        stage_pp_in(s, z_in, N, a, &a.lp_in);
+        stage_pp_out(s, z_out, (size_t)z_out->ld * N, (size_t)N, a);
+        stage_rng(s, rng, D, N, false, &a.rng);
+        stage_stats(s, stats, N, &a.st);
+    });
+    if (rc) return rc;
+    if ((rc = ensure(ctx, ctx->energy_ws, (size_t)(n_steps + 1) * (size_t)N * sizeof(double), "the multinomial energy tape")))
+        return rc;
+    a.energies = (double*)ctx->energy_ws.p;
     int nl = 0;
     CU(launch_multinomial(a, ctx->stream, &nl));
     ctx->launches += nl;
@@ -1793,31 +1690,19 @@ int ahmc_adapt_summary_f64(ahmc_ctx* ctx, int32_t D, int64_t N, const double* th
     if (D < 1 || N < 1 || ld < D) return fail(ctx, AHMC_ERR_INVALID, "need D >= 1, N >= 1, ld >= D");
     DeviceGuard g(ctx->device);
     const int blocks = (int)(N < ctx->sm_count ? N : ctx->sm_count);
-    const size_t need = ((size_t)blocks * (D + 1) + 2) * sizeof(double);
-    if (need > ctx->adapt_scratch_bytes) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->adapt_scratch);
-        ctx->adapt_scratch = nullptr;
-        ctx->adapt_scratch_bytes = 0;
-        if (cudaMalloc((void**)&ctx->adapt_scratch, need) != cudaSuccess)
-            return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for the adaptor workspace failed", need);
-        ctx->adapt_scratch_bytes = need;
-        CU(cudaMemsetAsync(ctx->adapt_scratch, 0, need, ctx->stream));
-    }
-    Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
-    st.reserve((size_t)ld * N * 8);
-    st.reserve((size_t)N * 8);
-    st.reserve((size_t)(2 + 2 * D) * 8);
-    int rc = st.prepare();
+    unsigned* counter;
+    double* partial;
+    int rc = summary_workspace(ctx, D, blocks, &counter, &partial);
     if (rc) return rc;
+    Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
     const double *d_theta, *d_alpha;
     double* d_out;
-    if ((rc = st.in(theta, (size_t)ld * N, &d_theta))) return rc;
-    if ((rc = st.in(acceptance_rate, (size_t)N, &d_alpha))) return rc;
-    if ((rc = st.out(out, (size_t)(2 + 2 * D), &d_out))) return rc;
-    // workspace: [counter (as 2 doubles)] [partials]
-    unsigned* counter = (unsigned*)ctx->adapt_scratch;
-    double* partial = ctx->adapt_scratch + 2;
+    rc = st.stage([&](Stager& s) {
+        s.in(theta, (size_t)ld * N, &d_theta);
+        s.in(acceptance_rate, (size_t)N, &d_alpha);
+        s.out(out, (size_t)(2 + 2 * D), &d_out);
+    });
+    if (rc) return rc;
     int nl = 0;
     CU(launch_adapt_summary(D, N, d_theta, ld, d_alpha, d_out, partial, counter, blocks, ctx->stream, &nl));
     ctx->launches += nl;
@@ -1830,16 +1715,14 @@ int ahmc_adapt_cov_f64(ahmc_ctx* ctx, int32_t D, int64_t N, const double* theta,
     if (D < 1 || N < 1 || ld < D) return fail(ctx, AHMC_ERR_INVALID, "need D >= 1, N >= 1, ld >= D");
     DeviceGuard g(ctx->device);
     Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
-    st.reserve((size_t)ld * N * 8);
-    st.reserve((size_t)D * 8);
-    st.reserve((size_t)D * D * 8);
-    int rc = st.prepare();
-    if (rc) return rc;
     const double *d_theta, *d_mean;
     double* d_out;
-    if ((rc = st.in(theta, (size_t)ld * N, &d_theta))) return rc;
-    if ((rc = st.in(mean, (size_t)D, &d_mean))) return rc;
-    if ((rc = st.out(out, (size_t)D * D, &d_out))) return rc;
+    int rc = st.stage([&](Stager& s) {
+        s.in(theta, (size_t)ld * N, &d_theta);
+        s.in(mean, (size_t)D, &d_mean);
+        s.out(out, (size_t)D * D, &d_out);
+    });
+    if (rc) return rc;
     int nl = 0;
     CU(launch_adapt_cov(D, N, d_theta, ld, d_mean, d_out, ctx->stream, &nl));
     ctx->launches += nl;
@@ -1862,27 +1745,26 @@ int ahmc_find_good_stepsize_f64(ahmc_ctx* ctx, const ahmc_model* model, const ah
     if (N == 0) return AHMC_OK;
     DeviceGuard g(ctx->device);
     Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
-    const size_t cin = (size_t)z->ld * N;
-    reserve_metric(st, metric, D, N);
-    st.reserve(cin * 8); st.reserve(cin * 8); st.reserve(cin * 8); st.reserve((size_t)D * N * 8);
-    st.reserve((size_t)N * 8); st.reserve((size_t)N * 8);
-    if ((rc = st.prepare())) return rc;
     FindEpsArgs a{};
     a.model = model_dev(model);
-    if ((rc = stage_metric(st, metric, D, N, &a.metric))) return rc;
     a.D = D;
     a.N = N;
     a.ld = z->ld;
-    if ((rc = st.in((const double*)z->theta, cin, &a.th))) return rc;
-    if ((rc = st.in((const double*)z->lp_gradient, cin, &a.g))) return rc;
-    if ((rc = st.in((const double*)z->lp_value, (size_t)N, &a.lp))) return rc;
-    if ((rc = st.in(rng->normal_tape, (size_t)D * N, &a.normal_tape))) return rc;
     a.seed = rng->seed;
     a.offset = rng->offset;
     a.eps0 = initial_step_size;
     a.max_iters = max_n_iters;
-    if ((rc = st.out(eps_out, (size_t)N, &a.eps_out))) return rc;
-    if ((rc = st.out(r_out, cin, &a.r_out))) return rc;
+    rc = st.stage([&](Stager& s) {
+        const size_t c = (size_t)z->ld * N;
+        stage_metric(s, metric, D, N, &a.metric);
+        s.in((const double*)z->theta, c, &a.th);
+        s.in((const double*)z->lp_gradient, c, &a.g);
+        s.in((const double*)z->lp_value, (size_t)N, &a.lp);
+        s.in(rng->normal_tape, (size_t)D * N, &a.normal_tape);
+        s.out(eps_out, (size_t)N, &a.eps_out);
+        s.out(r_out, c, &a.r_out);
+    });
+    if (rc) return rc;
     if (D > 512 && (rc = chain_workspace(ctx, (size_t)kBigFindEpsVectors * D * (size_t)N * sizeof(double), &a.scratch))) return rc;
     int nl = 0;
     CU(launch_find_eps(a, ctx->stream, &nl));
@@ -1899,11 +1781,10 @@ struct ahmc_comm {
 struct ahmc_pooled {
     int D = 0;
     int64_t N = 0;
-    char* dev = nullptr;  // one allocation: state | record | gathered (grown on demand) ...
+    void* dev = nullptr;  // one allocation: state | eps_chain | minv | w_mu | w_M2 | record | merged
     void* state = nullptr;
     double *eps_chain = nullptr, *minv = nullptr, *w_mu = nullptr, *w_M2 = nullptr, *record = nullptr, *merged = nullptr;
-    double* gathered = nullptr;
-    int gathered_ranks = 0;
+    DevBuf gathered;  // every rank's record (more than one rank)
 };
 
 int ahmc_comm_unique_id(ahmc_ctx* ctx, void* id128_out) {
@@ -1973,21 +1854,24 @@ int ahmc_pooled_create(ahmc_ctx* ctx, int32_t D, int64_t N, const ahmc_pooled_cf
     if (!a) return fail(ctx, AHMC_ERR_NOMEM, "out of host memory");
     a->D = D;
     a->N = N;
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
     const size_t rec = (size_t)(2 + 2 * D) * 8;
-    const size_t total = al(pooled_state_bytes()) + al((size_t)N * 8) + 3 * al((size_t)D * 8) + 2 * al(rec);
-    if (cudaMalloc((void**)&a->dev, total) != cudaSuccess) {
+    auto layout = [&](Carver& c) {
+        a->state = c.take<char>(pooled_state_bytes());
+        a->eps_chain = c.take<double>((size_t)N);
+        a->minv = c.take<double>((size_t)D);
+        a->w_mu = c.take<double>((size_t)D);
+        a->w_M2 = c.take<double>((size_t)D);
+        a->record = c.take<double>((size_t)(2 + 2 * D));
+        a->merged = c.take<double>((size_t)(2 + 2 * D));
+    };
+    Carver size;
+    layout(size);
+    if (cudaMalloc(&a->dev, size.off) != cudaSuccess) {
         delete a;
-        return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for the pooled adaptor failed", total);
+        return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for the pooled adaptor failed", size.off);
     }
-    char* p = a->dev;
-    a->state = p; p += al(pooled_state_bytes());
-    a->eps_chain = (double*)p; p += al((size_t)N * 8);
-    a->minv = (double*)p; p += al((size_t)D * 8);
-    a->w_mu = (double*)p; p += al((size_t)D * 8);
-    a->w_M2 = (double*)p; p += al((size_t)D * 8);
-    a->record = (double*)p; p += al(rec);
-    a->merged = (double*)p;
+    Carver c{(char*)a->dev};
+    layout(c);
     std::vector<char> img(pooled_state_bytes());
     pooled_state_init(img.data(), cfg->eps0, sched, cfg->delta, cfg->gamma, cfg->t0, cfg->kappa, cfg->n_adapts,
                       cfg->adapt_metric, cfg->n_min);
@@ -2008,7 +1892,7 @@ int ahmc_pooled_destroy(ahmc_ctx* ctx, ahmc_pooled* a) {
     DeviceGuard g(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     cudaFree(a->dev);
-    cudaFree(a->gathered);
+    cudaFree(a->gathered.p);
     delete a;
     return AHMC_OK;
 }
@@ -2023,35 +1907,20 @@ int ahmc_adapt_exchange_f64(ahmc_ctx* ctx, ahmc_comm* comm, ahmc_pooled* a, int3
     DeviceGuard g(ctx->device);
     const int R = comm ? comm->nranks : 1;
     const size_t rec = (size_t)(2 + 2 * D);
-    if (R > 1 && a->gathered_ranks < R) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        cudaFree(a->gathered);
-        a->gathered = nullptr;
-        if (cudaMalloc((void**)&a->gathered, rec * 8 * (size_t)R) != cudaSuccess)
-            return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc for the gathered records failed");
-        a->gathered_ranks = R;
-    }
-    // K5: this rank's record (same workspace discipline as ahmc_adapt_summary_f64)
+    int rc;
+    if (R > 1 && (rc = ensure(ctx, a->gathered, rec * 8 * (size_t)R, "the gathered records"))) return rc;
+    // K5: this rank's record
     const int blocks = (int)(N < ctx->sm_count ? N : ctx->sm_count);
-    const size_t need = ((size_t)blocks * (D + 1) + 2) * sizeof(double);
-    if (need > ctx->adapt_scratch_bytes) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->adapt_scratch);
-        ctx->adapt_scratch = nullptr;
-        ctx->adapt_scratch_bytes = 0;
-        if (cudaMalloc((void**)&ctx->adapt_scratch, need) != cudaSuccess)
-            return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc(%zu) for the adaptor workspace failed", need);
-        ctx->adapt_scratch_bytes = need;
-        CU(cudaMemsetAsync(ctx->adapt_scratch, 0, need, ctx->stream));
-    }
+    unsigned* counter;
+    double* partial;
+    if ((rc = summary_workspace(ctx, D, blocks, &counter, &partial))) return rc;
     int nl = 0;
-    CU(launch_adapt_summary(D, N, theta, ld, acceptance_rate, a->record, ctx->adapt_scratch + 2, (unsigned*)ctx->adapt_scratch,
-                            blocks, ctx->stream, &nl));
+    CU(launch_adapt_summary(D, N, theta, ld, acceptance_rate, a->record, partial, counter, blocks, ctx->stream, &nl));
     const double* gathered = a->record;
     if (R > 1) {
-        int rc = nccl_allgather_f64(a->record, a->gathered, rec, comm->nccl, ctx->stream);
-        if (rc) return fail(ctx, AHMC_ERR_CUDA, "ncclAllGather: %s", nccl_err(rc));
-        gathered = a->gathered;
+        if ((rc = nccl_allgather_f64(a->record, (double*)a->gathered.p, rec, comm->nccl, ctx->stream)))
+            return fail(ctx, AHMC_ERR_CUDA, "ncclAllGather: %s", nccl_err(rc));
+        gathered = (double*)a->gathered.p;
     }
     CU(launch_pooled_update(a->state, gathered, R, D, a->w_mu, a->w_M2, a->minv, a->eps_chain, N, eps_trace, a->merged,
                             ctx->stream, &nl));

@@ -573,10 +573,21 @@ static bool contig_ok(const LeapfrogArgs& a) {
     return true;
 }
 
+// one group of G lanes per chain, kBlockThreads per CTA; dynamic shared memory beyond 48 KB needs the kernel's opt-in
+template <class Args>
+static cudaError_t launch_warps(void (*kernel)(Args), long long N, int G, size_t smem, cudaStream_t st, const Args& a) {
+    const int chains_per_block = kBlockThreads / G;
+    const long long blocks = (N + chains_per_block - 1) / chains_per_block;
+    if (smem > 48 * 1024) {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+    }
+    kernel<<<(unsigned)blocks, kBlockThreads, smem, st>>>(a);
+    return cudaGetLastError();
+}
+
 template <int MODEL, int METRIC, int G, int E, bool CONTIG>
 static cudaError_t launch_lf_c(const LeapfrogArgs& a, cudaStream_t st) {
-    const int chains_per_block = kBlockThreads / G;
-    const long long blocks = (a.N + chains_per_block - 1) / chains_per_block;
     size_t sm = smem_bytes(MODEL, METRIC, a.D, G);
     const int occ = a.resident_blocks_per_sm;
     if (occ > 0) {
@@ -585,13 +596,7 @@ static cudaError_t launch_lf_c(const LeapfrogArgs& a, cudaStream_t st) {
         const size_t pad = (size_t)(227 * 1024) / (size_t)occ - 1024;
         if (pad > sm) sm = pad;
     }
-    if (sm > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(leapfrog_kernel<MODEL, METRIC, G, E, CONTIG>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        if (e != cudaSuccess) return e;
-    }
-    leapfrog_kernel<MODEL, METRIC, G, E, CONTIG><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
-    return cudaGetLastError();
+    return launch_warps(leapfrog_kernel<MODEL, METRIC, G, E, CONTIG>, a.N, G, sm, st, a);
 }
 template <int MODEL, int METRIC, int G, int E>
 static cudaError_t launch_lf_t(const LeapfrogArgs& a, cudaStream_t st) {
@@ -603,41 +608,15 @@ static cudaError_t launch_lf_t(const LeapfrogArgs& a, cudaStream_t st) {
 }
 template <int MODEL, int METRIC, int G, int E>
 static cudaError_t launch_fe_t(const FindEpsArgs& a, cudaStream_t st) {
-    const int chains_per_block = kBlockThreads / G;
-    const long long blocks = (a.N + chains_per_block - 1) / chains_per_block;
-    size_t sm = smem_bytes(MODEL, METRIC, a.D, G);
-    if (sm > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(find_eps_kernel<MODEL, METRIC, G, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        if (e != cudaSuccess) return e;
-    }
-    find_eps_kernel<MODEL, METRIC, G, E><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
-    return cudaGetLastError();
+    return launch_warps(find_eps_kernel<MODEL, METRIC, G, E>, a.N, G, smem_bytes(MODEL, METRIC, a.D, G), st, a);
 }
 template <int MODEL, int METRIC, int G, int E>
 static cudaError_t launch_pp_t(const PhasepointArgs& a, cudaStream_t st) {
-    const int chains_per_block = kBlockThreads / G;
-    const long long blocks = (a.N + chains_per_block - 1) / chains_per_block;
-    size_t sm = smem_bytes(MODEL, METRIC, a.D, G);
-    if (sm > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(phasepoint_kernel<MODEL, METRIC, G, E>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        if (e != cudaSuccess) return e;
-    }
-    phasepoint_kernel<MODEL, METRIC, G, E><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
-    return cudaGetLastError();
+    return launch_warps(phasepoint_kernel<MODEL, METRIC, G, E>, a.N, G, smem_bytes(MODEL, METRIC, a.D, G), st, a);
 }
 template <int MODEL, int METRIC, int G, int E, int ADAPT = 0>
 static cudaError_t launch_hmc_t(const HmcArgs& a, cudaStream_t st) {
-    const int chains_per_block = kBlockThreads / G;
-    const long long blocks = (a.lf.N + chains_per_block - 1) / chains_per_block;
-    size_t sm = smem_bytes(MODEL, METRIC, a.lf.D, G);
-    if (sm > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(hmc_kernel<MODEL, METRIC, G, E, ADAPT>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        if (e != cudaSuccess) return e;
-    }
-    hmc_kernel<MODEL, METRIC, G, E, ADAPT><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
-    return cudaGetLastError();
+    return launch_warps(hmc_kernel<MODEL, METRIC, G, E, ADAPT>, a.lf.N, G, smem_bytes(MODEL, METRIC, a.lf.D, G), st, a);
 }
 template <int FORM, int MODEL, int METRIC, int G, int E>
 static cudaError_t launch_hmc_adapt_t(const HmcArgs& a, cudaStream_t st) {
@@ -645,38 +624,19 @@ static cudaError_t launch_hmc_adapt_t(const HmcArgs& a, cudaStream_t st) {
 }
 template <int METRIC, int G, int E>
 static cudaError_t launch_kd_t(const SplitArgs& a, cudaStream_t st) {
-    const long long blocks = (a.N + kBlockThreads / G - 1) / (kBlockThreads / G);
-    size_t sm = smem_bytes(AHMC_MODEL_STD_NORMAL, METRIC, a.D, G);
-    if (sm > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(kick_drift_kernel<METRIC, G, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        if (e != cudaSuccess) return e;
-    }
-    kick_drift_kernel<METRIC, G, E><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
-    return cudaGetLastError();
+    return launch_warps(kick_drift_kernel<METRIC, G, E>, a.N, G, smem_bytes(AHMC_MODEL_STD_NORMAL, METRIC, a.D, G), st, a);
 }
 template <int METRIC, int G, int E>
 static cudaError_t launch_ke_t(const SplitArgs& a, cudaStream_t st) {
-    const long long blocks = (a.N + kBlockThreads / G - 1) / (kBlockThreads / G);
-    size_t sm = smem_bytes(AHMC_MODEL_STD_NORMAL, METRIC, a.D, G);
-    if (sm > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(kick_energy_kernel<METRIC, G, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        if (e != cudaSuccess) return e;
-    }
-    kick_energy_kernel<METRIC, G, E><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
-    return cudaGetLastError();
+    return launch_warps(kick_energy_kernel<METRIC, G, E>, a.N, G, smem_bytes(AHMC_MODEL_STD_NORMAL, METRIC, a.D, G), st, a);
 }
 template <int DUMMY, int G, int E>
 static cudaError_t launch_mh_t(const MhArgs& a, cudaStream_t st) {
-    const long long blocks = (a.N + kBlockThreads / G - 1) / (kBlockThreads / G);
-    mh_select_kernel<G, E><<<(unsigned)blocks, kBlockThreads, 0, st>>>(a);
-    return cudaGetLastError();
+    return launch_warps(mh_select_kernel<G, E>, a.N, G, 0, st, a);
 }
 template <int METRIC, int G, int E>
 static cudaError_t launch_mom_t(const MomentumArgs& a, cudaStream_t st) {
-    const int chains_per_block = kBlockThreads / G;
-    const long long blocks = (a.N + chains_per_block - 1) / chains_per_block;
-    momentum_kernel<METRIC, G, E><<<(unsigned)blocks, kBlockThreads, 0, st>>>(a);
-    return cudaGetLastError();
+    return launch_warps(momentum_kernel<METRIC, G, E>, a.N, G, 0, st, a);
 }
 
 #define AHMC_DISPATCH_LAYOUT(FN, ...)                                   \
@@ -763,75 +723,53 @@ static cudaError_t mom_layout(const MomentumArgs& a, cudaStream_t st, int G, int
         return cudaErrorInvalidValue;                                                                   \
     } while (0)
 
-cudaError_t launch_leapfrog(const LeapfrogArgs& a, cudaStream_t st, int* n_launches) {
+// the entry points with a D > 512 streaming form and a run-time compiled form: past D = 512 `big`, for a user target its
+// compiled kernel `uk` (estimator form `form`), else `builtin(G, E)` at the register-resident layout of D
+template <class Args, class Builtin>
+static cudaError_t front_door(const Args& a, int D, long long N, const ModelDev& model, const MetricDev& metric,
+                              cudaError_t (*big)(const Args&, cudaStream_t), int uk, int form, cudaStream_t st,
+                              int* n_launches, Builtin&& builtin) {
     int G, E;
-    if (a.D > 512) {  // beyond the register-resident layouts: the streaming form (ahmc_bigd.cu)
+    if (D > 512) {  // beyond the register-resident layouts: the streaming form (ahmc_bigd.cu, ahmc_bigd_hmc.cu)
         if (n_launches) *n_launches += 1;
-        return launch_leapfrog_big(a, st);
+        return big(a, st);
     }
-    if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
+    if (!pick_layout(D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
-    if (a.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
+    if (model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
         const int cpb = kBlockThreads / G;
-        return user_launch((UserModule*)a.model.user, UK_LEAPFROG, metric_form(a.metric), G, E, &a, (unsigned)((a.N + cpb - 1) / cpb),
-                           smem_bytes(AHMC_MODEL_USER, a.metric.kind, a.D, G), st);
+        return user_launch((UserModule*)model.user, uk, metric_form(metric), G, E, &a, (unsigned)((N + cpb - 1) / cpb),
+                           smem_bytes(AHMC_MODEL_USER, metric.kind, D, G), st, form);
     }
-    AHMC_DISPATCH_MM(lf_layout, a.model.kind, metric_form(a.metric));
+    return builtin(G, E);
+}
+
+cudaError_t launch_leapfrog(const LeapfrogArgs& a, cudaStream_t st, int* n_launches) {
+    return front_door(a, a.D, a.N, a.model, a.metric, launch_leapfrog_big, UK_LEAPFROG, 0, st, n_launches,
+                      [&](int G, int E) { AHMC_DISPATCH_MM(lf_layout, a.model.kind, metric_form(a.metric)); });
 }
 
 cudaError_t launch_find_eps(const FindEpsArgs& a, cudaStream_t st, int* n_launches) {
-    int G, E;
-    if (a.D > 512) {  // beyond the register-resident layouts: the streaming form (ahmc_bigd_hmc.cu)
-        if (n_launches) *n_launches += 1;
-        return launch_find_eps_big(a, st);
-    }
-    if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
-    if (n_launches) *n_launches += 1;
-    if (a.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
-        const int cpb = kBlockThreads / G;
-        return user_launch((UserModule*)a.model.user, UK_FIND_EPS, metric_form(a.metric), G, E, &a, (unsigned)((a.N + cpb - 1) / cpb),
-                           smem_bytes(AHMC_MODEL_USER, a.metric.kind, a.D, G), st);
-    }
-    AHMC_DISPATCH_MM(fe_layout, a.model.kind, metric_form(a.metric));
+    return front_door(a, a.D, a.N, a.model, a.metric, launch_find_eps_big, UK_FIND_EPS, 0, st, n_launches,
+                      [&](int G, int E) { AHMC_DISPATCH_MM(fe_layout, a.model.kind, metric_form(a.metric)); });
 }
 
 cudaError_t launch_phasepoint(const PhasepointArgs& a, cudaStream_t st, int* n_launches) {
-    int G, E;
-    if (a.D > 512) {
-        if (n_launches) *n_launches += 1;
-        return launch_phasepoint_big(a, st);
-    }
-    if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
-    if (n_launches) *n_launches += 1;
-    if (a.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
-        const int cpb = kBlockThreads / G;
-        return user_launch((UserModule*)a.model.user, UK_PHASEPOINT, metric_form(a.metric), G, E, &a, (unsigned)((a.N + cpb - 1) / cpb),
-                           smem_bytes(AHMC_MODEL_USER, a.metric.kind, a.D, G), st);
-    }
-    AHMC_DISPATCH_MM(pp_layout, a.model.kind, metric_form(a.metric));
+    return front_door(a, a.D, a.N, a.model, a.metric, launch_phasepoint_big, UK_PHASEPOINT, 0, st, n_launches,
+                      [&](int G, int E) { AHMC_DISPATCH_MM(pp_layout, a.model.kind, metric_form(a.metric)); });
 }
 
 cudaError_t launch_hmc(const HmcArgs& a, cudaStream_t st, int* n_launches) {
-    int G, E;
-    if (a.lf.D > 512) {
-        if (n_launches) *n_launches += 1;
-        return launch_hmc_big(a, st);
-    }
-    if (!pick_layout(a.lf.D, &G, &E)) return cudaErrorInvalidValue;
-    if (n_launches) *n_launches += 1;
-    if (a.lf.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
-        const int cpb = kBlockThreads / G;
-        return user_launch((UserModule*)a.lf.model.user, a.ad.enabled ? UK_HMC_ADAPT : UK_HMC, metric_form(a.lf.metric), G, E, &a,
-                           (unsigned)((a.lf.N + cpb - 1) / cpb), smem_bytes(AHMC_MODEL_USER, a.lf.metric.kind, a.lf.D, G), st,
-                           a.ad.enabled ? adapt_form(a.ad) : 0);
-    }
-    if (a.ad.enabled) {  // the adaptive forms: Diag metric (diagonal estimators) or Dense metric (WelfordCov form)
-        if (a.lf.metric.kind == AHMC_METRIC_DENSE) return hmc_adapt_model<AHMC_ADAPT_WELFORD_COV>(a, st, G, E);
-        if (a.lf.metric.kind != AHMC_METRIC_DIAG) return cudaErrorInvalidValue;
-        return adapt_form(a.ad) == AHMC_ADAPT_NUTPIE ? hmc_adapt_model<AHMC_ADAPT_NUTPIE>(a, st, G, E)
-                                                     : hmc_adapt_model<AHMC_ADAPT_WELFORD>(a, st, G, E);
-    }
-    AHMC_DISPATCH_MM(hmc_layout, a.lf.model.kind, metric_form(a.lf.metric));
+    return front_door(a, a.lf.D, a.lf.N, a.lf.model, a.lf.metric, launch_hmc_big, a.ad.enabled ? UK_HMC_ADAPT : UK_HMC,
+                      a.ad.enabled ? adapt_form(a.ad) : 0, st, n_launches, [&](int G, int E) -> cudaError_t {
+        if (a.ad.enabled) {  // the adaptive forms: Diag metric (diagonal estimators) or Dense metric (WelfordCov form)
+            if (a.lf.metric.kind == AHMC_METRIC_DENSE) return hmc_adapt_model<AHMC_ADAPT_WELFORD_COV>(a, st, G, E);
+            if (a.lf.metric.kind != AHMC_METRIC_DIAG) return cudaErrorInvalidValue;
+            return adapt_form(a.ad) == AHMC_ADAPT_NUTPIE ? hmc_adapt_model<AHMC_ADAPT_NUTPIE>(a, st, G, E)
+                                                         : hmc_adapt_model<AHMC_ADAPT_WELFORD>(a, st, G, E);
+        }
+        AHMC_DISPATCH_MM(hmc_layout, a.lf.model.kind, metric_form(a.lf.metric));
+    });
 }
 
 cudaError_t launch_kick_drift(const SplitArgs& a, cudaStream_t st, int* n_launches) {
