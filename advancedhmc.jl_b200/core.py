@@ -478,7 +478,8 @@ def dHdr(h: Hamiltonian, r):
 # ------------------------------------------------------------------------------------------------
 class PhiloxRNG:
     """Counter-based generator living on the device (Philox4x32-10 keyed by seed; one `offset` tick per
-    transition).  Replaces the reference's `AbstractRNG` / vector of RNGs (src/utilities.jl:5-23)."""
+    transition).  Replaces the reference's `AbstractRNG` / vector of RNGs (src/utilities.jl:5-23).  The counter holds
+    offsets below 2^36: a launch that would pass that bound is refused (InvalidArgument)."""
 
     def __init__(self, seed: int = 0):
         self.seed, self.offset = int(seed) & (2**64 - 1), 0

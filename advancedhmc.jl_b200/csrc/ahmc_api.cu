@@ -271,6 +271,16 @@ int check_philox_d(ahmc_ctx* ctx, int32_t D) {
     if (D >= (1 << 25)) return fail(ctx, AHMC_ERR_INVALID, "D=%d: Philox momentum draws need D < 2^25", D);
     return AHMC_OK;
 }
+// the transition offset fills bits 24..59 of the counter's high word, below the stream id: a launch that draws from the
+// Philox streams at offsets offset .. offset + n_transitions - 1 must stay below 2^36, or its counters are another
+// stream's (the normals at offset 3 * 2^36 would be the exponentials at offset 0)
+static int check_philox_offset(ahmc_ctx* ctx, uint64_t offset, int64_t n_transitions) {
+    constexpr uint64_t kOffsets = 1ull << 36;
+    if (offset > kOffsets || (uint64_t)n_transitions > kOffsets - offset)
+        return fail(ctx, AHMC_ERR_INVALID, "Philox offset %llu + %lld transitions passes 2^36: the counter holds offsets below 2^36",
+                    (unsigned long long)offset, (long long)n_transitions);
+    return AHMC_OK;
+}
 
 int check_pp(ahmc_ctx* ctx, const ahmc_phasepoint* z, int32_t D, const char* name, bool need_cache, int64_t N) {
     if (!z) return fail(ctx, AHMC_ERR_INVALID, "%s is NULL", name);
@@ -1214,6 +1224,7 @@ int ahmc_rand_momentum_f64(ahmc_ctx* ctx, const ahmc_metric* metric, int32_t D, 
     if (!ctx || !metric || !rng || !r) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/metric/rng/r");
     int rc = check_common(ctx, nullptr, metric, D, N, true);
     if (!rc && !rng->normal_tape) rc = check_philox_d(ctx, D);
+    if (!rc && !rng->normal_tape) rc = check_philox_offset(ctx, rng->offset, 1);
     if (rc) return rc;
     if (ld < D) return fail(ctx, AHMC_ERR_INVALID, "ld < D");
     if (metric->kind == AHMC_METRIC_DENSE && !metric->cholU)
@@ -1409,6 +1420,8 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
     rc = check_common(ctx, model, metric, D, N, true);
     if (!rc && D > 512 && rng->temper_alpha > 0.0) rc = fail(ctx, AHMC_ERR_UNSUPPORTED, "TemperedLeapfrog at D > 512 is not built");
     if (!rc && D > 512 && !(flags & AHMC_FLAG_NO_REFRESH) && !rng->normal_tape) rc = check_philox_d(ctx, D);
+    if (!rc && (!rng->exp_tape || (!(flags & AHMC_FLAG_NO_REFRESH) && !rng->normal_tape)))
+        rc = check_philox_offset(ctx, rng->offset, n_transitions);
     if (rc) return rc;
     if ((rc = check_pp(ctx, z_in, D, "z_in", true, N))) return rc;
     if ((rc = check_pp(ctx, z_out, D, "z_out", true, N))) return rc;
@@ -1492,6 +1505,8 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
     if (n_transitions > 1 && (rng->normal_tape || rng->exp_tape || rng->dir_tape))
         return fail(ctx, AHMC_ERR_INVALID, "random tapes describe ONE transition; multi-transition sampling uses the Philox streams");
     if ((rc = check_refresh_rng(ctx, rng))) return rc;
+    // (every NUTS launch: a tree that outgrows its exponential or direction tape continues on the Philox streams)
+    if ((rc = check_philox_offset(ctx, rng->offset, n_transitions))) return rc;
     if ((rc = check_common(ctx, model, metric, D, N))) return rc;
     if ((rc = check_pp(ctx, z_in, D, "z_in", true, N))) return rc;
     if ((rc = check_pp(ctx, z_out, D, "z_out", true, N))) return rc;
@@ -1610,6 +1625,8 @@ int ahmc_hmc_multinomial_transition_f64(ahmc_ctx* ctx, const ahmc_model* model, 
         return fail(ctx, AHMC_ERR_UNSUPPORTED, "MultinomialTS static transitions: built-in targets only");
     if ((rc = check_transition_io(ctx, metric, z_out, flags))) return rc;
     if ((rc = check_refresh_rng(ctx, rng))) return rc;
+    if ((!rng->exp_tape || (!(flags & AHMC_FLAG_NO_REFRESH) && !rng->normal_tape)) && (rc = check_philox_offset(ctx, rng->offset, 1)))
+        return rc;
     if (N == 0) return AHMC_OK;
     DeviceGuard g(ctx->device);
     Stager st(ctx, flags & AHMC_FLAG_HOST_BUFFERS);
@@ -1735,6 +1752,7 @@ int ahmc_find_good_stepsize_f64(ahmc_ctx* ctx, const ahmc_model* model, const ah
     if (!ctx || !model || !metric || !rng || !eps_out) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/model/metric/rng/eps_out");
     int rc = check_common(ctx, model, metric, D, N, true);
     if (!rc && D > 512 && !rng->normal_tape) rc = check_philox_d(ctx, D);
+    if (!rc && !rng->normal_tape) rc = check_philox_offset(ctx, rng->offset, 1);
     if (rc) return rc;
     if (!z || (N > 0 && (!z->theta || !z->lp_value || !z->lp_gradient)))
         return fail(ctx, AHMC_ERR_INVALID, "z.theta / lp_value / lp_gradient is NULL (call ahmc_phasepoint_f64 first)");

@@ -946,7 +946,8 @@ __device__ __forceinline__ bool leapfrog_step_lean(ChainState<E>& s, const Model
 }
 
 // ------------------------------------------------------------------------------------------------
-// counter-based RNG: Philox4x32-10 (Salmon et al. 2011), keyed by seed, counter = (chain, draw, stream, offset)
+// counter-based RNG: Philox4x32-10 (Salmon et al. 2011) keyed by the seed; the 128-bit counter of a draw is
+// (chain, (offset << 24) ^ (stream << 60) ^ block), injective while block < 2^24 and offset < 2^36 (DESIGN.md, "Random streams")
 // ------------------------------------------------------------------------------------------------
 struct Philox {
     static __device__ __forceinline__ void round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
@@ -973,7 +974,7 @@ struct Philox {
         out[2] = c[2];
         out[3] = c[3];
     }
-    // uniform in (0,1): 53 random bits, never 0 or 1
+    // uniform in (0,1]: 53 random bits plus a half, never 0; the half rounds to even above 2^52, so the all-ones draw is 1.0
     static __device__ __forceinline__ double u01(uint32_t a, uint32_t b) {
         uint64_t x = (((uint64_t)a << 32) | b) >> 11;  // 53 bits
         return ((double)x + 0.5) * (1.0 / 9007199254740992.0);
@@ -983,17 +984,6 @@ struct Philox {
 // stream ids for the counter's high word
 constexpr uint64_t STREAM_NORMAL = 1, STREAM_EXP = 2, STREAM_DIR = 3;
 
-// standard normal for (chain, coordinate d) of transition `offset` (Box-Muller on one Philox block:
-// one block yields two normals; coordinate d uses block d/2, component d%2)
-__device__ __forceinline__ double philox_normal(uint64_t seed, uint64_t offset, long long chain, int d) {
-    uint32_t o[4];
-    Philox::gen(seed, (uint64_t)chain, (offset << 24) ^ (STREAM_NORMAL << 60) ^ (uint64_t)(d >> 1), o);
-    double u1 = Philox::u01(o[0], o[1]), u2 = Philox::u01(o[2], o[3]);
-    double rad = sqrt(-2.0 * log(u1));
-    double s, c;
-    sincospi(2.0 * u2, &s, &c);
-    return (d & 1) ? rad * s : rad * c;
-}
 // D standard normals of (chain, transition) as a group-distributed vector: coordinates e = 2q and e = 2q+1 of a lane
 // share ONE Philox block and ONE Box-Muller evaluation (block index = lane + G*q), so a lane with E coordinates
 // spends ceil(E/2) blocks.  The stream is a pure function of (seed, offset, chain, D) -- the layout (G) follows from D.

@@ -121,7 +121,10 @@ typedef struct ahmc_stats {
  * the value comes from the built-in counter-based Philox4x32-10 generator keyed by (seed, chain, draw). */
 typedef struct ahmc_rng {
     uint64_t seed;
-    uint64_t offset;           /* transition counter: advance by 1 per transition call */
+    uint64_t offset;           /* transition counter: advance by 1 per transition call (n_transitions per multi-transition
+                                  launch).  A call that draws from the Philox streams needs offset + n_transitions <= 2^36
+                                  (AHMC_ERR_INVALID otherwise); every NUTS call counts, since a tree that outgrows its
+                                  tapes continues on the streams. */
     const double* normal_tape; /* D x N standard normals for rand_momentum (metric.jl:290-320) */
     const double* exp_tape;    /* static: N; NUTS: exp_stride x N, consumed in the reference's order */
     int64_t exp_stride;
