@@ -5,6 +5,7 @@
 // Targets: std-normal, diagonal Gaussian, Neal's funnel; metrics: Unit, Diag (shared or per chain).  Dense operators at
 // D > 512 need the tiled GEMM form inside a CTA-per-tile kernel and are reported as unsupported.
 #include "ahmc_bigd.cuh"
+#include "ahmc_dispatch.cuh"
 
 namespace ahmc {
 
@@ -90,18 +91,15 @@ bool bigd_supported(int model_kind, int metric_kind) {
            (metric_kind == AHMC_METRIC_UNIT || metric_kind == AHMC_METRIC_DIAG);
 }
 
-
 cudaError_t launch_leapfrog_big(const LeapfrogArgs& a, cudaStream_t st) {
     if (!bigd_supported(a.model.kind, a.metric.kind) || a.temper_alpha > 0.0) return cudaErrorNotSupported;
-    const unsigned blocks = (unsigned)((a.N + kBlockThreads / 32 - 1) / (kBlockThreads / 32));
-    AHMC_BIG_DISPATCH(leapfrog_big_kernel, a.model.kind, a.metric.kind, a);
-    return cudaGetLastError();
+    return with_model_metric(BigModels{}, BigMetrics{}, a.model.kind, a.metric.kind,
+                             [&](auto M, auto K) { return launch_warps(leapfrog_big_kernel<M, K>, a.N, 32, 0, st, a); }, cudaErrorNotSupported);
 }
 cudaError_t launch_phasepoint_big(const PhasepointArgs& a, cudaStream_t st) {
     if (!bigd_supported(a.model.kind, a.metric.kind)) return cudaErrorNotSupported;
-    const unsigned blocks = (unsigned)((a.N + kBlockThreads / 32 - 1) / (kBlockThreads / 32));
-    AHMC_BIG_DISPATCH(phasepoint_big_kernel, a.model.kind, a.metric.kind, a);
-    return cudaGetLastError();
+    return with_model_metric(BigModels{}, BigMetrics{}, a.model.kind, a.metric.kind,
+                             [&](auto M, auto K) { return launch_warps(phasepoint_big_kernel<M, K>, a.N, 32, 0, st, a); }, cudaErrorNotSupported);
 }
 
 }  // namespace ahmc

@@ -163,23 +163,4 @@ __device__ __forceinline__ bool big_step(const BigModel<MODEL>& mo, const double
     return f;
 }
 
-// launch KERNEL<model, metric> (bigd_supported combinations) with one warp per chain; `blocks` and `st` in scope
-#define AHMC_BIG_DISPATCH(KERNEL, model_kind, metric_kind, ...)                                                      \
-    do {                                                                                                             \
-        const bool diag = (metric_kind) == AHMC_METRIC_DIAG;                                                         \
-        switch (model_kind) {                                                                                        \
-            case AHMC_MODEL_STD_NORMAL:                                                                              \
-                if (diag) KERNEL<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__); \
-                else KERNEL<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_UNIT><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__);      \
-                break;                                                                                               \
-            case AHMC_MODEL_DIAG_GAUSS:                                                                              \
-                if (diag) KERNEL<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__); \
-                else KERNEL<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__);      \
-                break;                                                                                               \
-            default:                                                                                                 \
-                if (diag) KERNEL<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__);     \
-                else KERNEL<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT><<<blocks, kBlockThreads, 0, st>>>(__VA_ARGS__);          \
-        }                                                                                                            \
-    } while (0)
-
 }  // namespace ahmc

@@ -11,6 +11,9 @@
 //   find_eps:    r0, then the probe's theta, r, g (the start theta and g stay in the read-only input).
 #include "ahmc_bigd.cuh"
 #include "ahmc_chain_adapt.cuh"
+#ifndef AHMC_SIMT_EMULATION
+#include "ahmc_dispatch.cuh"
+#endif
 
 namespace ahmc {
 
@@ -216,8 +219,7 @@ __global__ void __launch_bounds__(kBlockThreads) hmc_big_kernel(const HmcArgs h)
         // mh_accept_ratio + accept_phasepoint! + momentum flip (trajectory.jl:283, 312-332, 869-877)
         const double H1 = -(lp + lk);
         const bool accept = H1 < H0 + ex;
-        double alpha = exp(H0 - H1);  // min(1, exp(H - H')) with Julia's NaN-propagating min
-        alpha = (alpha != alpha) ? alpha : (alpha < 1.0 ? alpha : 1.0);
+        const double alpha = mh_accept_ratio(H0, H1);
         double* dro = h.draws ? h.draws + si * D : nullptr;
         for (int d0 = 0; d0 < D; d0 += kBigTile) {
             double tt[kBigE], rr[kBigE];
@@ -247,14 +249,7 @@ __global__ void __launch_bounds__(kBlockThreads) hmc_big_kernel(const HmcArgs h)
             a.lk_out[chain] = lkn;
             if (a.status) a.status[chain] = fin ? 0u : AHMC_STATUS_NONFINITE;
             if (a.steps_done) a.steps_done[chain] = steps;
-            const StatsDev& st = h.st;
-            if (st.n_steps) st.n_steps[si] = a.n_steps;  // nsteps(tau), nominal (trajectory.jl:288)
-            if (st.is_accept) st.is_accept[si] = accept ? 1 : 0;
-            if (st.acceptance_rate) st.acceptance_rate[si] = alpha;
-            if (st.log_density) st.log_density[si] = lpn;
-            if (st.hamiltonian_energy) st.hamiltonian_energy[si] = H;
-            if (st.hamiltonian_energy_error) st.hamiltonian_energy_error[si] = H - H0;
-            if (st.numerical_error) st.numerical_error[si] = finite_d(H1) ? 0 : 1;
+            record_stats(h.st, si, a.n_steps, accept, alpha, lpn, H, H0, !finite_d(H1));  // nsteps(tau), nominal (trajectory.jl:288)
         }
         if constexpr (ADAPT != 0) {  // iteration t + 1 of `sample` (sampler.jl:182)
             __syncwarp();
@@ -332,43 +327,28 @@ __global__ void __launch_bounds__(kBlockThreads) find_eps_big_kernel(const FindE
 }
 
 #ifndef AHMC_SIMT_EMULATION  // host launch code (skipped by the CPU SIMT emulation harness, tests/simt_emu/)
-static unsigned big_blocks(long long N) { return (unsigned)((N + kBlockThreads / 32 - 1) / (kBlockThreads / 32)); }
-
 cudaError_t launch_rand_momentum_big(const MomentumArgs& a, cudaStream_t st) {
-    const unsigned blocks = big_blocks(a.N);
-    if (a.metric.kind == AHMC_METRIC_DIAG) momentum_big_kernel<AHMC_METRIC_DIAG><<<blocks, kBlockThreads, 0, st>>>(a);
-    else if (a.metric.kind == AHMC_METRIC_UNIT) momentum_big_kernel<AHMC_METRIC_UNIT><<<blocks, kBlockThreads, 0, st>>>(a);
-    else return cudaErrorNotSupported;
-    return cudaGetLastError();
-}
-
-template <int FORM>
-static void launch_hmc_big_adapt(const HmcArgs& a, unsigned blocks, cudaStream_t st) {
-    switch (a.lf.model.kind) {
-        case AHMC_MODEL_STD_NORMAL: hmc_big_kernel<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG, FORM><<<blocks, kBlockThreads, 0, st>>>(a); break;
-        case AHMC_MODEL_DIAG_GAUSS: hmc_big_kernel<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, FORM><<<blocks, kBlockThreads, 0, st>>>(a); break;
-        default: hmc_big_kernel<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG, FORM><<<blocks, kBlockThreads, 0, st>>>(a);
-    }
+    return with_kind(BigMetrics{}, a.metric.kind, [&](auto K) { return launch_warps(momentum_big_kernel<K>, a.N, 32, 0, st, a); },
+                     cudaErrorNotSupported);
 }
 
 cudaError_t launch_hmc_big(const HmcArgs& a, cudaStream_t st) {
-    if (!bigd_supported(a.lf.model.kind, a.lf.metric.kind) || a.rng.temper_alpha > 0.0) return cudaErrorNotSupported;
-    const unsigned blocks = big_blocks(a.lf.N);
-    if (a.ad.enabled) {  // the adaptive form: Diag metric only (the chain adapts its diagonal M^-1)
-        if (a.lf.metric.kind != AHMC_METRIC_DIAG) return cudaErrorInvalidValue;
-        if (adapt_form(a.ad) == AHMC_ADAPT_NUTPIE) launch_hmc_big_adapt<AHMC_ADAPT_NUTPIE>(a, blocks, st);
-        else launch_hmc_big_adapt<AHMC_ADAPT_WELFORD>(a, blocks, st);
-        return cudaGetLastError();
-    }
-    AHMC_BIG_DISPATCH(hmc_big_kernel, a.lf.model.kind, a.lf.metric.kind, a);
-    return cudaGetLastError();
+    const LeapfrogArgs& lf = a.lf;
+    if (!bigd_supported(lf.model.kind, lf.metric.kind) || a.rng.temper_alpha > 0.0) return cudaErrorNotSupported;
+    auto run = [&](auto form, auto metrics) {
+        return with_model_metric(BigModels{}, metrics, lf.model.kind, lf.metric.kind,
+                                 [&](auto M, auto K) { return launch_warps(hmc_big_kernel<M, K, form>, lf.N, 32, 0, st, a); });
+    };
+    if (!a.ad.enabled) return run(IC<0>{}, BigMetrics{});
+    // the adaptive form: Diag metric only (the chain adapts its diagonal M^-1)
+    if (adapt_form(a.ad) == AHMC_ADAPT_NUTPIE) return run(IC<AHMC_ADAPT_NUTPIE>{}, Kinds<AHMC_METRIC_DIAG>{});
+    return run(IC<AHMC_ADAPT_WELFORD>{}, Kinds<AHMC_METRIC_DIAG>{});
 }
 
 cudaError_t launch_find_eps_big(const FindEpsArgs& a, cudaStream_t st) {
     if (!bigd_supported(a.model.kind, a.metric.kind)) return cudaErrorNotSupported;
-    const unsigned blocks = big_blocks(a.N);
-    AHMC_BIG_DISPATCH(find_eps_big_kernel, a.model.kind, a.metric.kind, a);
-    return cudaGetLastError();
+    return with_model_metric(BigModels{}, BigMetrics{}, a.model.kind, a.metric.kind,
+                             [&](auto M, auto K) { return launch_warps(find_eps_big_kernel<M, K>, a.N, 32, 0, st, a); }, cudaErrorNotSupported);
 }
 #endif  // AHMC_SIMT_EMULATION
 

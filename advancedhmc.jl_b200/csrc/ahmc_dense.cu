@@ -13,10 +13,10 @@
 // proof as the separable fast path applies with the induced infinity norms (K = (1+|eps| |Minv|_inf)(1+|eps| |P|_inf)),
 // energies are evaluated once at the end, and a tile that fails a magnitude check is handed, chain by chain, to
 // the exact warp-per-chain kernel (`only_mask`) inside the same stream -- no host round trip.
-#include <cstdlib>
-#include <cstring>
-
 #include "ahmc_kernels.cuh"
+#ifndef AHMC_SIMT_EMULATION
+#include "ahmc_dispatch.cuh"
+#endif
 
 namespace ahmc {
 
@@ -412,17 +412,12 @@ cudaError_t launch_vec_norm(const double* v, int D, double* norm, cudaStream_t s
     return cudaGetLastError();
 }
 
-
 template <int RB, int CB, int MINB = 1>
 static cudaError_t launch_dense_t(const DenseArgs& a, cudaStream_t st) {
     constexpr int CT = 8 * CB;
     const int Ds = a.Dp + 4;
     const size_t sm = ((size_t)kStages * kKC * Ds + (size_t)CT * Ds + 8 * CT * 2) * sizeof(double) + 64;
-    cudaError_t e = cudaFuncSetAttribute(dense_traj_kernel<RB, CB, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    if (e != cudaSuccess) return e;
-    const long long blocks = (a.N + CT - 1) / CT;
-    dense_traj_kernel<RB, CB, MINB><<<(unsigned)blocks, kDenseThreads, sm, st>>>(a);
-    return cudaGetLastError();
+    return launch_kernel(dense_traj_kernel<RB, CB, MINB>, (a.N + CT - 1) / CT, kDenseThreads, sm, st, a);
 }
 
 cudaError_t launch_dense_traj(const DenseTrajHost& h, cudaStream_t st, int* n_launches) {
@@ -436,13 +431,8 @@ cudaError_t launch_dense_traj(const DenseTrajHost& h, cudaStream_t st, int* n_la
     const int RB = h.Dp / 64;
     switch (RB) {
         case 1: return launch_dense_t<1, 4>(a, st);
-        case 2: {
-            // D <= 128: tiles of 16 chains, two CTAs per SM -- the barrier / copy waits of one hide behind the other.
-            // AHMC_DENSE_TILE=32x1 selects the single-CTA form (one 32-chain CTA per SM) for A/B runs.
-            const char* ev = getenv("AHMC_DENSE_TILE");
-            if (ev && !strcmp(ev, "32x1")) return launch_dense_t<2, 4>(a, st);
-            return launch_dense_t<2, 2, 2>(a, st);
-        }
+        case 2: return launch_dense_t<2, 2, 2>(a, st);  // D <= 128: tiles of 16 chains, two CTAs per SM -- the barrier / copy
+                                                         // waits of one hide behind the other
         case 3: return launch_dense_t<3, 2>(a, st);
         case 4: return launch_dense_t<4, 2>(a, st);
         case 5: return launch_dense_t<5, 1>(a, st);

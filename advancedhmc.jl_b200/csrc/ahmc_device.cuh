@@ -1003,6 +1003,24 @@ __device__ __forceinline__ void philox_normals(uint64_t seed, uint64_t offset, l
     }
 }
 
+// rand_momentum (metric.jl:290-320) of a chain: standard normals from the tape (D x N, ld = D) or the chain's Philox
+// stream of transition `offset`, scaled by the metric
+template <int METRIC, int G, int E>
+__device__ __forceinline__ void draw_momentum(const MetricOps<METRIC, G, E>& me, const double* normal_tape, uint64_t seed,
+                                              uint64_t offset, long long chain, int l, int D, double (&r)[E]) {
+    if (normal_tape) vload_nc<G, E>(r, normal_tape + (long long)D * chain, l, D);
+    else philox_normals<G, E>(seed, offset, chain, l, D, r);
+    me.rand_momentum(r, l);
+}
+
+// min(0, x) and min(1, x) with Julia's NaN-propagating min
+__device__ __forceinline__ double jl_min0(double x) { return (x != x) ? x : (x < 0.0 ? x : 0.0); }
+// mh_accept_ratio's acceptance probability min(1, exp(H - H')) (trajectory.jl:869-877)
+__device__ __forceinline__ double mh_accept_ratio(double H0, double H1) {
+    const double alpha = exp(H0 - H1);
+    return (alpha != alpha) ? alpha : (alpha < 1.0 ? alpha : 1.0);
+}
+
 // standard exponential, k-th draw of (chain, transition)
 __device__ __forceinline__ double philox_exp(uint64_t seed, uint64_t offset, long long chain, int k) {
     uint32_t o[4];

@@ -86,6 +86,19 @@ struct RngDev {
     double temper_alpha;   // > 0: the transition integrates with TemperedLeapfrog(eps, alpha) (integrator.jl:174-209)
 };
 
+// the statistics every transition records at entry si (trajectory.jl:288-300); the tree samplers add tree_depth and
+// max_hamiltonian_energy_error themselves.  H: energy of the new phase point, H0: of the start point
+__device__ __forceinline__ void record_stats(const StatsDev& st, long long si, int n_steps, bool accept, double alpha, double lp,
+                                             double H, double H0, bool numerical_error) {
+    if (st.n_steps) st.n_steps[si] = n_steps;
+    if (st.is_accept) st.is_accept[si] = accept ? 1 : 0;
+    if (st.acceptance_rate) st.acceptance_rate[si] = alpha;
+    if (st.log_density) st.log_density[si] = lp;
+    if (st.hamiltonian_energy) st.hamiltonian_energy[si] = H;
+    if (st.hamiltonian_energy_error) st.hamiltonian_energy_error[si] = H - H0;
+    if (st.numerical_error) st.numerical_error[si] = numerical_error ? 1 : 0;
+}
+
 // in-kernel per-chain adaptation (adaptive K2 / K3 forms, ahmc_chain_adapt.cuh): NesterovDualAveraging + a windowed
 // WelfordVar, NutpieVar or (Dense metric) WelfordCov per chain
 struct AdaptDev {

@@ -26,9 +26,13 @@
 #include "ahmc_chain_adapt.cuh"
 #include "ahmc_kernels.cuh"
 #include "ahmc_traj.cuh"
+#if !defined(AHMC_SIMT_EMULATION) && !defined(__CUDACC_RTC__)
+#include "ahmc_dispatch.cuh"
+#endif
 
 namespace ahmc {
 
+// the register-resident layout of D; with_layout (ahmc_dispatch.cuh) instantiates the kernels for exactly these 8 pairs
 bool pick_layout(int D, int* G, int* E) {
     if (D < 1) return false;
     if (D <= 4) { *G = 4; *E = 1; return true; }
@@ -164,8 +168,7 @@ struct HmcIO {
         const LeapfrogArgs& a = h.lf;
         const double H1 = -(lp + lk);                   // energy(z') (hamiltonian.jl:149,194)
         const bool accept = H1 < H0 + ex;               // trajectory.jl:869-877
-        double alpha = exp(H0 - H1);                    // min(1, exp(H - H')) with Julia's NaN-propagating min
-        alpha = (alpha != alpha) ? alpha : (alpha < 1.0 ? alpha : 1.0);
+        const double alpha = mh_accept_ratio(H0, H1);
         double* tho = a.th_out + a.ld_out * chain;
         double* ro = a.r_out + a.ld_out * chain;
         double* go = a.g_out + a.ld_out * chain;
@@ -200,14 +203,7 @@ struct HmcIO {
             a.lk_out[chain] = lkn;
             if (a.status) a.status[chain] = fin ? 0u : AHMC_STATUS_NONFINITE;
             if (a.steps_done) a.steps_done[chain] = steps;
-            const StatsDev& st = h.st;
-            if (st.n_steps) st.n_steps[stat_idx] = a.n_steps;  // nsteps(tau), nominal (trajectory.jl:288)
-            if (st.is_accept) st.is_accept[stat_idx] = accept ? 1 : 0;
-            if (st.acceptance_rate) st.acceptance_rate[stat_idx] = alpha;
-            if (st.log_density) st.log_density[stat_idx] = lpn;
-            if (st.hamiltonian_energy) st.hamiltonian_energy[stat_idx] = H;
-            if (st.hamiltonian_energy_error) st.hamiltonian_energy_error[stat_idx] = H - H0;
-            if (st.numerical_error) st.numerical_error[stat_idx] = finite_d(H1) ? 0 : 1;
+            record_stats(h.st, stat_idx, a.n_steps, accept, alpha, lpn, H, H0, !finite_d(H1));  // nsteps(tau), nominal (trajectory.jl:288)
         }
         this->alpha = alpha;
         (void)dr;
@@ -252,12 +248,7 @@ __global__ void __launch_bounds__(kBlockThreads, min_blocks_hmc<MODEL, METRIC, E
         // refresh (hamiltonian.jl:213-220): new momentum, kinetic energy; lp is the cached value (quirk Q2:
         // the reference recomputes it from theta -- same number)
         if (h.refresh) {
-            if (h.rng.normal_tape) {
-                vload_nc<G, E>(io.r0, h.rng.normal_tape + (long long)D * chain, l, D);
-            } else {
-                philox_normals<G, E>(h.rng.seed, off, chain, l, D, io.r0);
-            }
-            me.rand_momentum(io.r0, l);
+            draw_momentum(me, h.rng.normal_tape, h.rng.seed, off, chain, l, D, io.r0);
             if (h.rng.partial_alpha != 0.0) {  // PartialMomentumRefreshment (hamiltonian.jl:243-254)
                 double rp[E];
                 vload_nc<G, E>(rp, first ? a.r_in + a.ld_in * chain : a.r_out + a.ld_out * chain, l, D);
@@ -317,9 +308,7 @@ __global__ void __launch_bounds__(kBlockThreads) find_eps_kernel(const FindEpsAr
     ChainState<E> z0;
     vload_nc<G, E>(z0.th, a.th + a.ld * chain, l, D);
     vload_nc<G, E>(z0.g, a.g + a.ld * chain, l, D);
-    if (a.normal_tape) vload_nc<G, E>(z0.r, a.normal_tape + (long long)D * chain, l, D);
-    else philox_normals<G, E>(a.seed, a.offset, chain, l, D, z0.r);
-    me.rand_momentum(z0.r, l);
+    draw_momentum(me, a.normal_tape, a.seed, a.offset, chain, l, D, z0.r);
     if (a.r_out && valid) vstore<G, E>(a.r_out + a.ld * chain, z0.r, l, D);
     double dr[E];
     const double lk0 = map_nonfinite(kinetic<METRIC, G, E>(me, z0.r, dr, xs, l));
@@ -406,12 +395,7 @@ __global__ void __launch_bounds__(kBlockThreads) momentum_kernel(const MomentumA
     MetricOps<METRIC, G, E> me;
     me.load(a.metric, chain, l, D);
     double r[E];
-    if (a.normal_tape) {
-        vload_nc<G, E>(r, a.normal_tape + (long long)D * chain, l, D);
-    } else {
-        philox_normals<G, E>(a.seed, a.offset, chain, l, D, r);
-    }
-    me.rand_momentum(r, l);
+    draw_momentum(me, a.normal_tape, a.seed, a.offset, chain, l, D, r);
     if (valid) vstore<G, E>(a.r + a.ld * chain, r, l, D);
 }
 
@@ -520,8 +504,7 @@ __global__ void __launch_bounds__(kBlockThreads) mh_select_kernel(const MhArgs a
     const double H0 = -(lp0 + lk0), H1 = -(lp1 + lk1);
     const double ex = a.rng.exp_tape ? a.rng.exp_tape[chain] : philox_exp(a.rng.seed, a.rng.offset, chain, 0);
     const bool accept = H1 < H0 + ex;
-    double alpha = exp(H0 - H1);
-    alpha = (alpha != alpha) ? alpha : (alpha < 1.0 ? alpha : 1.0);
+    const double alpha = mh_accept_ratio(H0, H1);
     double t[E];
     if (accept) {
         vload_nc<G, E>(t, a.r + a.ld * chain, l, D);
@@ -543,14 +526,7 @@ __global__ void __launch_bounds__(kBlockThreads) mh_select_kernel(const MhArgs a
         const double H = -(lpn + lkn);
         a.lp[chain] = lpn;
         a.lk[chain] = lkn;
-        const StatsDev& st = a.st;
-        if (st.n_steps) st.n_steps[chain] = a.n_steps;
-        if (st.is_accept) st.is_accept[chain] = accept ? 1 : 0;
-        if (st.acceptance_rate) st.acceptance_rate[chain] = alpha;
-        if (st.log_density) st.log_density[chain] = lpn;
-        if (st.hamiltonian_energy) st.hamiltonian_energy[chain] = H;
-        if (st.hamiltonian_energy_error) st.hamiltonian_energy_error[chain] = H - H0;
-        if (st.numerical_error) st.numerical_error[chain] = finite_d(H1) ? 0 : 1;
+        record_stats(a.st, chain, a.n_steps, accept, alpha, lpn, H, H0, !finite_d(H1));
     }
 }
 
@@ -573,19 +549,6 @@ static bool contig_ok(const LeapfrogArgs& a) {
     return true;
 }
 
-// one group of G lanes per chain, kBlockThreads per CTA; dynamic shared memory beyond 48 KB needs the kernel's opt-in
-template <class Args>
-static cudaError_t launch_warps(void (*kernel)(Args), long long N, int G, size_t smem, cudaStream_t st, const Args& a) {
-    const int chains_per_block = kBlockThreads / G;
-    const long long blocks = (N + chains_per_block - 1) / chains_per_block;
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-    }
-    kernel<<<(unsigned)blocks, kBlockThreads, smem, st>>>(a);
-    return cudaGetLastError();
-}
-
 template <int MODEL, int METRIC, int G, int E, bool CONTIG>
 static cudaError_t launch_lf_c(const LeapfrogArgs& a, cudaStream_t st) {
     size_t sm = smem_bytes(MODEL, METRIC, a.D, G);
@@ -606,122 +569,6 @@ static cudaError_t launch_lf_t(const LeapfrogArgs& a, cudaStream_t st) {
     }
     return launch_lf_c<MODEL, METRIC, G, E, false>(a, st);
 }
-template <int MODEL, int METRIC, int G, int E>
-static cudaError_t launch_fe_t(const FindEpsArgs& a, cudaStream_t st) {
-    return launch_warps(find_eps_kernel<MODEL, METRIC, G, E>, a.N, G, smem_bytes(MODEL, METRIC, a.D, G), st, a);
-}
-template <int MODEL, int METRIC, int G, int E>
-static cudaError_t launch_pp_t(const PhasepointArgs& a, cudaStream_t st) {
-    return launch_warps(phasepoint_kernel<MODEL, METRIC, G, E>, a.N, G, smem_bytes(MODEL, METRIC, a.D, G), st, a);
-}
-template <int MODEL, int METRIC, int G, int E, int ADAPT = 0>
-static cudaError_t launch_hmc_t(const HmcArgs& a, cudaStream_t st) {
-    return launch_warps(hmc_kernel<MODEL, METRIC, G, E, ADAPT>, a.lf.N, G, smem_bytes(MODEL, METRIC, a.lf.D, G), st, a);
-}
-template <int FORM, int MODEL, int METRIC, int G, int E>
-static cudaError_t launch_hmc_adapt_t(const HmcArgs& a, cudaStream_t st) {
-    return launch_hmc_t<MODEL, METRIC, G, E, FORM>(a, st);
-}
-template <int METRIC, int G, int E>
-static cudaError_t launch_kd_t(const SplitArgs& a, cudaStream_t st) {
-    return launch_warps(kick_drift_kernel<METRIC, G, E>, a.N, G, smem_bytes(AHMC_MODEL_STD_NORMAL, METRIC, a.D, G), st, a);
-}
-template <int METRIC, int G, int E>
-static cudaError_t launch_ke_t(const SplitArgs& a, cudaStream_t st) {
-    return launch_warps(kick_energy_kernel<METRIC, G, E>, a.N, G, smem_bytes(AHMC_MODEL_STD_NORMAL, METRIC, a.D, G), st, a);
-}
-template <int DUMMY, int G, int E>
-static cudaError_t launch_mh_t(const MhArgs& a, cudaStream_t st) {
-    return launch_warps(mh_select_kernel<G, E>, a.N, G, 0, st, a);
-}
-template <int METRIC, int G, int E>
-static cudaError_t launch_mom_t(const MomentumArgs& a, cudaStream_t st) {
-    return launch_warps(momentum_kernel<METRIC, G, E>, a.N, G, 0, st, a);
-}
-
-#define AHMC_DISPATCH_LAYOUT(FN, ...)                                   \
-    do {                                                                \
-        if (G == 4 && E == 1) return FN<__VA_ARGS__, 4, 1>(a, st);      \
-        if (G == 8 && E == 1) return FN<__VA_ARGS__, 8, 1>(a, st);      \
-        if (G == 16 && E == 1) return FN<__VA_ARGS__, 16, 1>(a, st);    \
-        if (G == 32 && E == 1) return FN<__VA_ARGS__, 32, 1>(a, st);    \
-        if (G == 32 && E == 2) return FN<__VA_ARGS__, 32, 2>(a, st);    \
-        if (G == 32 && E == 4) return FN<__VA_ARGS__, 32, 4>(a, st);    \
-        if (G == 32 && E == 8) return FN<__VA_ARGS__, 32, 8>(a, st);    \
-        if (G == 32 && E == 16) return FN<__VA_ARGS__, 32, 16>(a, st);  \
-        return cudaErrorInvalidValue;                                   \
-    } while (0)
-
-template <int MODEL, int METRIC>
-static cudaError_t lf_layout(const LeapfrogArgs& a, cudaStream_t st, int G, int E) {
-    AHMC_DISPATCH_LAYOUT(launch_lf_t, MODEL, METRIC);
-}
-template <int MODEL, int METRIC>
-static cudaError_t fe_layout(const FindEpsArgs& a, cudaStream_t st, int G, int E) {
-    AHMC_DISPATCH_LAYOUT(launch_fe_t, MODEL, METRIC);
-}
-template <int MODEL, int METRIC>
-static cudaError_t pp_layout(const PhasepointArgs& a, cudaStream_t st, int G, int E) {
-    AHMC_DISPATCH_LAYOUT(launch_pp_t, MODEL, METRIC);
-}
-template <int MODEL, int METRIC>
-static cudaError_t hmc_layout(const HmcArgs& a, cudaStream_t st, int G, int E) {
-    AHMC_DISPATCH_LAYOUT(launch_hmc_t, MODEL, METRIC);
-}
-template <int MODEL, int FORM>
-static cudaError_t hmc_adapt_layout(const HmcArgs& a, cudaStream_t st, int G, int E) {
-    // the metric the estimator adapts: Diag, or for WelfordCov the chain's own Dense rows
-    AHMC_DISPATCH_LAYOUT(launch_hmc_adapt_t, FORM, MODEL, FORM == AHMC_ADAPT_WELFORD_COV ? kMetricDenseChain : AHMC_METRIC_DIAG);
-}
-template <int FORM>
-static cudaError_t hmc_adapt_model(const HmcArgs& a, cudaStream_t st, int G, int E) {
-    switch (a.lf.model.kind) {
-        case AHMC_MODEL_STD_NORMAL: return hmc_adapt_layout<AHMC_MODEL_STD_NORMAL, FORM>(a, st, G, E);
-        case AHMC_MODEL_DIAG_GAUSS: return hmc_adapt_layout<AHMC_MODEL_DIAG_GAUSS, FORM>(a, st, G, E);
-        case AHMC_MODEL_DENSE_GAUSS: return hmc_adapt_layout<AHMC_MODEL_DENSE_GAUSS, FORM>(a, st, G, E);
-        case AHMC_MODEL_FUNNEL: return hmc_adapt_layout<AHMC_MODEL_FUNNEL, FORM>(a, st, G, E);
-    }
-    return cudaErrorInvalidValue;
-}
-template <int METRIC>
-static cudaError_t kd_layout(const SplitArgs& a, cudaStream_t st, int G, int E) {
-    AHMC_DISPATCH_LAYOUT(launch_kd_t, METRIC);
-}
-template <int METRIC>
-static cudaError_t ke_layout(const SplitArgs& a, cudaStream_t st, int G, int E) {
-    AHMC_DISPATCH_LAYOUT(launch_ke_t, METRIC);
-}
-template <int DUMMY>
-static cudaError_t mh_layout(const MhArgs& a, cudaStream_t st, int G, int E) {
-    AHMC_DISPATCH_LAYOUT(launch_mh_t, DUMMY);
-}
-template <int METRIC>
-static cudaError_t mom_layout(const MomentumArgs& a, cudaStream_t st, int G, int E) {
-    AHMC_DISPATCH_LAYOUT(launch_mom_t, METRIC);
-}
-
-#define AHMC_DISPATCH_MM(FN, model_kind, metric_kind)                                                   \
-    do {                                                                                                \
-        switch ((model_kind) * 4 + (metric_kind)) {                                                     \
-            case 0: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_UNIT>(a, st, G, E);                    \
-            case 1: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG>(a, st, G, E);                    \
-            case 2: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DENSE>(a, st, G, E);                   \
-            case 3: return FN<AHMC_MODEL_STD_NORMAL, kMetricDenseChain>(a, st, G, E);                   \
-            case 4: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);                    \
-            case 5: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);                    \
-            case 6: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);                   \
-            case 7: return FN<AHMC_MODEL_DIAG_GAUSS, kMetricDenseChain>(a, st, G, E);                   \
-            case 8: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);                   \
-            case 9: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);                   \
-            case 10: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);                 \
-            case 11: return FN<AHMC_MODEL_DENSE_GAUSS, kMetricDenseChain>(a, st, G, E);                 \
-            case 12: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT>(a, st, G, E);                       \
-            case 13: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG>(a, st, G, E);                       \
-            case 14: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DENSE>(a, st, G, E);                      \
-            case 15: return FN<AHMC_MODEL_FUNNEL, kMetricDenseChain>(a, st, G, E);                      \
-        }                                                                                               \
-        return cudaErrorInvalidValue;                                                                   \
-    } while (0)
 
 // the entry points with a D > 512 streaming form and a run-time compiled form: past D = 512 `big`, for a user target its
 // compiled kernel `uk` (estimator form `form`), else `builtin(G, E)` at the register-resident layout of D
@@ -745,79 +592,81 @@ static cudaError_t front_door(const Args& a, int D, long long N, const ModelDev&
 }
 
 cudaError_t launch_leapfrog(const LeapfrogArgs& a, cudaStream_t st, int* n_launches) {
-    return front_door(a, a.D, a.N, a.model, a.metric, launch_leapfrog_big, UK_LEAPFROG, 0, st, n_launches,
-                      [&](int G, int E) { AHMC_DISPATCH_MM(lf_layout, a.model.kind, metric_form(a.metric)); });
+    return front_door(a, a.D, a.N, a.model, a.metric, launch_leapfrog_big, UK_LEAPFROG, 0, st, n_launches, [&](int G, int E) {
+        return with_model_metric_layout(AllModels{}, AllMetrics{}, a.model.kind, metric_form(a.metric), G, E,
+                                        [&](auto M, auto K, auto g, auto e) { return launch_lf_t<M, K, g, e>(a, st); });
+    });
 }
 
 cudaError_t launch_find_eps(const FindEpsArgs& a, cudaStream_t st, int* n_launches) {
-    return front_door(a, a.D, a.N, a.model, a.metric, launch_find_eps_big, UK_FIND_EPS, 0, st, n_launches,
-                      [&](int G, int E) { AHMC_DISPATCH_MM(fe_layout, a.model.kind, metric_form(a.metric)); });
+    return front_door(a, a.D, a.N, a.model, a.metric, launch_find_eps_big, UK_FIND_EPS, 0, st, n_launches, [&](int G, int E) {
+        return with_model_metric_layout(AllModels{}, AllMetrics{}, a.model.kind, metric_form(a.metric), G, E, [&](auto M, auto K, auto g, auto e) {
+            return launch_warps(find_eps_kernel<M, K, g, e>, a.N, g, smem_bytes(M, K, a.D, g), st, a);
+        });
+    });
 }
 
 cudaError_t launch_phasepoint(const PhasepointArgs& a, cudaStream_t st, int* n_launches) {
-    return front_door(a, a.D, a.N, a.model, a.metric, launch_phasepoint_big, UK_PHASEPOINT, 0, st, n_launches,
-                      [&](int G, int E) { AHMC_DISPATCH_MM(pp_layout, a.model.kind, metric_form(a.metric)); });
+    return front_door(a, a.D, a.N, a.model, a.metric, launch_phasepoint_big, UK_PHASEPOINT, 0, st, n_launches, [&](int G, int E) {
+        return with_model_metric_layout(AllModels{}, AllMetrics{}, a.model.kind, metric_form(a.metric), G, E, [&](auto M, auto K, auto g, auto e) {
+            return launch_warps(phasepoint_kernel<M, K, g, e>, a.N, g, smem_bytes(M, K, a.D, g), st, a);
+        });
+    });
 }
 
 cudaError_t launch_hmc(const HmcArgs& a, cudaStream_t st, int* n_launches) {
-    return front_door(a, a.lf.D, a.lf.N, a.lf.model, a.lf.metric, launch_hmc_big, a.ad.enabled ? UK_HMC_ADAPT : UK_HMC,
+    const LeapfrogArgs& lf = a.lf;
+    return front_door(a, lf.D, lf.N, lf.model, lf.metric, launch_hmc_big, a.ad.enabled ? UK_HMC_ADAPT : UK_HMC,
                       a.ad.enabled ? adapt_form(a.ad) : 0, st, n_launches, [&](int G, int E) -> cudaError_t {
-        if (a.ad.enabled) {  // the adaptive forms: Diag metric (diagonal estimators) or Dense metric (WelfordCov form)
-            if (a.lf.metric.kind == AHMC_METRIC_DENSE) return hmc_adapt_model<AHMC_ADAPT_WELFORD_COV>(a, st, G, E);
-            if (a.lf.metric.kind != AHMC_METRIC_DIAG) return cudaErrorInvalidValue;
-            return adapt_form(a.ad) == AHMC_ADAPT_NUTPIE ? hmc_adapt_model<AHMC_ADAPT_NUTPIE>(a, st, G, E)
-                                                         : hmc_adapt_model<AHMC_ADAPT_WELFORD>(a, st, G, E);
-        }
-        AHMC_DISPATCH_MM(hmc_layout, a.lf.model.kind, metric_form(a.lf.metric));
+        auto run = [&](auto form, auto metrics, int metric) {
+            return with_model_metric_layout(AllModels{}, metrics, lf.model.kind, metric, G, E, [&](auto M, auto K, auto g, auto e) {
+                return launch_warps(hmc_kernel<M, K, g, e, form>, lf.N, g, smem_bytes(M, K, lf.D, g), st, a);
+            });
+        };
+        if (!a.ad.enabled) return run(IC<0>{}, AllMetrics{}, metric_form(lf.metric));
+        // the adaptive forms run on the metric their estimator adapts: Diag, or for WelfordCov the chain's own Dense rows
+        if (lf.metric.kind == AHMC_METRIC_DENSE) return run(IC<AHMC_ADAPT_WELFORD_COV>{}, Kinds<kMetricDenseChain>{}, kMetricDenseChain);
+        if (adapt_form(a.ad) == AHMC_ADAPT_NUTPIE) return run(IC<AHMC_ADAPT_NUTPIE>{}, Kinds<AHMC_METRIC_DIAG>{}, lf.metric.kind);
+        return run(IC<AHMC_ADAPT_WELFORD>{}, Kinds<AHMC_METRIC_DIAG>{}, lf.metric.kind);
+    });
+}
+
+// the kernels without a model (split step, momentum draw): f(METRIC, G, E) for the metric form, at the layout of D
+template <class F>
+static cudaError_t metric_layout(int D, const MetricDev& metric, int* n_launches, F&& f) {
+    int G, E;
+    if (!pick_layout(D, &G, &E)) return cudaErrorInvalidValue;
+    if (n_launches) *n_launches += 1;
+    return with_kind(AllMetrics{}, metric_form(metric), [&](auto K) {
+        return with_layout(G, E, [&](auto g, auto e) { return f(K, g, e); });
     });
 }
 
 cudaError_t launch_kick_drift(const SplitArgs& a, cudaStream_t st, int* n_launches) {
-    int G, E;
-    if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
-    if (n_launches) *n_launches += 1;
-    switch (metric_form(a.metric)) {
-        case AHMC_METRIC_UNIT: return kd_layout<AHMC_METRIC_UNIT>(a, st, G, E);
-        case AHMC_METRIC_DIAG: return kd_layout<AHMC_METRIC_DIAG>(a, st, G, E);
-        case AHMC_METRIC_DENSE: return kd_layout<AHMC_METRIC_DENSE>(a, st, G, E);
-        case kMetricDenseChain: return kd_layout<kMetricDenseChain>(a, st, G, E);
-    }
-    return cudaErrorInvalidValue;
+    return metric_layout(a.D, a.metric, n_launches, [&](auto K, auto g, auto e) {
+        return launch_warps(kick_drift_kernel<K, g, e>, a.N, g, smem_bytes(AHMC_MODEL_STD_NORMAL, K, a.D, g), st, a);
+    });
 }
 cudaError_t launch_kick_energy(const SplitArgs& a, cudaStream_t st, int* n_launches) {
-    int G, E;
-    if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
-    if (n_launches) *n_launches += 1;
-    switch (metric_form(a.metric)) {
-        case AHMC_METRIC_UNIT: return ke_layout<AHMC_METRIC_UNIT>(a, st, G, E);
-        case AHMC_METRIC_DIAG: return ke_layout<AHMC_METRIC_DIAG>(a, st, G, E);
-        case AHMC_METRIC_DENSE: return ke_layout<AHMC_METRIC_DENSE>(a, st, G, E);
-        case kMetricDenseChain: return ke_layout<kMetricDenseChain>(a, st, G, E);
-    }
-    return cudaErrorInvalidValue;
+    return metric_layout(a.D, a.metric, n_launches, [&](auto K, auto g, auto e) {
+        return launch_warps(kick_energy_kernel<K, g, e>, a.N, g, smem_bytes(AHMC_MODEL_STD_NORMAL, K, a.D, g), st, a);
+    });
 }
 cudaError_t launch_mh_select(const MhArgs& a, cudaStream_t st, int* n_launches) {
     int G, E;
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
-    return mh_layout<0>(a, st, G, E);
+    return with_layout(G, E, [&](auto g, auto e) { return launch_warps(mh_select_kernel<g, e>, a.N, g, 0, st, a); });
 }
 
 cudaError_t launch_rand_momentum(const MomentumArgs& a, cudaStream_t st, int* n_launches) {
-    int G, E;
     if (a.D > 512) {
         if (n_launches) *n_launches += 1;
         return launch_rand_momentum_big(a, st);
     }
-    if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
-    if (n_launches) *n_launches += 1;
-    switch (metric_form(a.metric)) {
-        case AHMC_METRIC_UNIT: return mom_layout<AHMC_METRIC_UNIT>(a, st, G, E);
-        case AHMC_METRIC_DIAG: return mom_layout<AHMC_METRIC_DIAG>(a, st, G, E);
-        case AHMC_METRIC_DENSE: return mom_layout<AHMC_METRIC_DENSE>(a, st, G, E);
-        case kMetricDenseChain: return mom_layout<kMetricDenseChain>(a, st, G, E);
-    }
-    return cudaErrorInvalidValue;
+    return metric_layout(a.D, a.metric, n_launches, [&](auto K, auto g, auto e) {
+        return launch_warps(momentum_kernel<K, g, e>, a.N, g, 0, st, a);
+    });
 }
 
 #endif  // AHMC_SIMT_EMULATION

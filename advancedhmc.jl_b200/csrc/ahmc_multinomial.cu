@@ -9,9 +9,10 @@
 //    z, zs_fwd...)`); here only the n+1 ENERGIES are kept (per-chain scratch), the index is selected, and the
 //    chosen point is re-materialised by re-running that many steps from z: same arithmetic, same bits, no
 //    O(n * D) trajectory storage.
-#include <cstdio>
-
 #include "ahmc_kernels.cuh"
+#ifndef AHMC_SIMT_EMULATION
+#include "ahmc_dispatch.cuh"
+#endif
 
 namespace ahmc {
 
@@ -37,7 +38,7 @@ __global__ void __launch_bounds__(kBlockThreads) trajectory_kernel(const TrajArg
     vload_nc<G, E>(s.th, a.th_in + a.ld_in * chain, l, D);
     vload_nc<G, E>(s.r, a.r_in + a.ld_in * chain, l, D);
     vload_nc<G, E>(s.g, a.g_in + a.ld_in * chain, l, D);
-    const double sa = a.temper_alpha > 0.0 ? sqrt(a.temper_alpha) : 1.0;
+    const double sa = a.temper_alpha > 0.0 ? sqrt(a.temper_alpha) : 1.0;  // (hoisted out of the step loop: not temper_muls)
     bool active = valid;
     int done = 0;
     for (int i = 1; i <= a.n_steps; ++i) {
@@ -66,8 +67,6 @@ __global__ void __launch_bounds__(kBlockThreads) trajectory_kernel(const TrajArg
 }
 
 // ------------------------------------------------------------------------------------------------ MultinomialTS static
-__device__ __forceinline__ double jl_min0m(double x) { return (x != x) ? x : (x < 0.0 ? x : 0.0); }
-
 template <int MODEL, int METRIC, int G, int E>
 __global__ void __launch_bounds__(kBlockThreads) multinomial_kernel(const MultinomialArgs a) {
     extern __shared__ double smem[];
@@ -89,9 +88,7 @@ __global__ void __launch_bounds__(kBlockThreads) multinomial_kernel(const Multin
     // z = refresh(rng, h, z) with the cached lp / gradient (hamiltonian.jl:213-220)
     double r0[E], dr[E];
     if (a.refresh) {
-        if (a.rng.normal_tape) vload_nc<G, E>(r0, a.rng.normal_tape + (long long)D * chain, l, D);
-        else philox_normals<G, E>(a.rng.seed, a.rng.offset, chain, l, D, r0);
-        me.rand_momentum(r0, l);
+        draw_momentum(me, a.rng.normal_tape, a.rng.seed, a.rng.offset, chain, l, D, r0);
         if (a.rng.partial_alpha != 0.0) {
             double rp[E];
             vload_nc<G, E>(rp, a.r_in + a.ld_in * chain, l, D);
@@ -176,7 +173,7 @@ __global__ void __launch_bounds__(kBlockThreads) multinomial_kernel(const Multin
         const double Hp = Hat(p);
         C += exp(-Hp - lse);                   // cumsum(P) (utilities.jl:101)
         if (C < u) ++cnt;                      // count(C .< u)
-        asum += exp(jl_min0m(-(Hp - H0)));     // alpha_i = exp(min(0, -dH)) (trajectory.jl:386-388)
+        asum += exp(jl_min0(-(Hp - H0)));     // alpha_i = exp(min(0, -dH)) (trajectory.jl:386-388)
     }
     int idx = cnt;
     if (idx > len - 1) idx = len - 1;
@@ -200,7 +197,7 @@ __global__ void __launch_bounds__(kBlockThreads) multinomial_kernel(const Multin
             const double H = -(s.lp + s.lk);
             a.lp_out[chain] = s.lp;
             a.lk_out[chain] = s.lk;
-            const StatsDev& st = a.st;
+            const StatsDev& st = a.st;  // (not record_stats: sharing it changes this kernel's generated code)
             if (st.n_steps) st.n_steps[chain] = a.n_steps;
             if (st.is_accept) st.is_accept[chain] = 1;
             if (st.acceptance_rate) st.acceptance_rate[chain] = alpha;
@@ -222,89 +219,23 @@ __global__ void __launch_bounds__(kBlockThreads) multinomial_kernel(const Multin
 
 // ------------------------------------------------------------------------------------------------ dispatch
 #ifndef AHMC_SIMT_EMULATION  // host launch code (skipped by the CPU SIMT emulation harness, tests/simt_emu/)
-template <int MODEL, int METRIC, int G, int E>
-static cudaError_t launch_traj_t(const TrajArgs& a, cudaStream_t st) {
-    const long long blocks = (a.N + kBlockThreads / G - 1) / (kBlockThreads / G);
-    size_t sm = smem_bytes(MODEL, METRIC, a.D, G);
-    if (sm > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(trajectory_kernel<MODEL, METRIC, G, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        if (e != cudaSuccess) return e;
-    }
-    trajectory_kernel<MODEL, METRIC, G, E><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
-    return cudaGetLastError();
-}
-template <int MODEL, int METRIC, int G, int E>
-static cudaError_t launch_mn_t(const MultinomialArgs& a, cudaStream_t st) {
-    const long long blocks = (a.N + kBlockThreads / G - 1) / (kBlockThreads / G);
-    size_t sm = smem_bytes(MODEL, METRIC, a.D, G);
-    if (sm > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(multinomial_kernel<MODEL, METRIC, G, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        if (e != cudaSuccess) return e;
-    }
-    multinomial_kernel<MODEL, METRIC, G, E><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) {
-        cudaFuncAttributes fa{};
-        cudaError_t ae = cudaFuncGetAttributes(&fa, multinomial_kernel<MODEL, METRIC, G, E>);
-        fprintf(stderr, "[ahmc] multinomial launch failed: %s | model=%d metric=%d G=%d E=%d blocks=%lld smem=%zu stream=%p | attr: %s regs=%d "
-                        "static_smem=%zu maxthreads=%d\n", cudaGetErrorString(le), MODEL, METRIC, G, E, blocks, sm, (void*)st,
-                cudaGetErrorString(ae), fa.numRegs, fa.sharedSizeBytes, fa.maxThreadsPerBlock);
-    }
-    return le;
-}
-
-#define AHMC_LAYOUTS(FN, ...)                                          \
-    do {                                                               \
-        if (G == 4 && E == 1) return FN<__VA_ARGS__, 4, 1>(a, st);     \
-        if (G == 8 && E == 1) return FN<__VA_ARGS__, 8, 1>(a, st);     \
-        if (G == 16 && E == 1) return FN<__VA_ARGS__, 16, 1>(a, st);   \
-        if (G == 32 && E == 1) return FN<__VA_ARGS__, 32, 1>(a, st);   \
-        if (G == 32 && E == 2) return FN<__VA_ARGS__, 32, 2>(a, st);   \
-        if (G == 32 && E == 4) return FN<__VA_ARGS__, 32, 4>(a, st);   \
-        if (G == 32 && E == 8) return FN<__VA_ARGS__, 32, 8>(a, st);   \
-        if (G == 32 && E == 16) return FN<__VA_ARGS__, 32, 16>(a, st); \
-        return cudaErrorInvalidValue;                                  \
-    } while (0)
-
-template <int MODEL, int METRIC>
-static cudaError_t traj_layout(const TrajArgs& a, cudaStream_t st, int G, int E) { AHMC_LAYOUTS(launch_traj_t, MODEL, METRIC); }
-template <int MODEL, int METRIC>
-static cudaError_t mn_layout(const MultinomialArgs& a, cudaStream_t st, int G, int E) { AHMC_LAYOUTS(launch_mn_t, MODEL, METRIC); }
-
-#define AHMC_MM(FN, mk, tk)                                                                   \
-    do {                                                                                      \
-        switch ((mk) * 4 + (tk)) {                                                        \
-            case 0: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_UNIT>(a, st, G, E);      \
-            case 1: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG>(a, st, G, E);      \
-            case 2: return FN<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DENSE>(a, st, G, E);     \
-            case 3: return FN<AHMC_MODEL_STD_NORMAL, kMetricDenseChain>(a, st, G, E);     \
-            case 4: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);      \
-            case 5: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);      \
-            case 6: return FN<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);     \
-            case 7: return FN<AHMC_MODEL_DIAG_GAUSS, kMetricDenseChain>(a, st, G, E);     \
-            case 8: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT>(a, st, G, E);     \
-            case 9: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG>(a, st, G, E);     \
-            case 10: return FN<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE>(a, st, G, E);   \
-            case 11: return FN<AHMC_MODEL_DENSE_GAUSS, kMetricDenseChain>(a, st, G, E);   \
-            case 12: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT>(a, st, G, E);         \
-            case 13: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG>(a, st, G, E);         \
-            case 14: return FN<AHMC_MODEL_FUNNEL, AHMC_METRIC_DENSE>(a, st, G, E);        \
-            case 15: return FN<AHMC_MODEL_FUNNEL, kMetricDenseChain>(a, st, G, E);        \
-        }                                                                                     \
-        return cudaErrorInvalidValue;                                                         \
-    } while (0)
-
-cudaError_t launch_trajectory(const TrajArgs& a, cudaStream_t st, int* n_launches) {
+// f(MODEL, METRIC, G, E) for a full-trajectory or multinomial launch
+template <class Args, class F>
+static cudaError_t traj_dispatch(const Args& a, int* n_launches, F&& f) {
     int G, E;
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
     if (n_launches) *n_launches += 1;
-    AHMC_MM(traj_layout, a.model.kind, metric_form(a.metric));
+    return with_model_metric_layout(AllModels{}, AllMetrics{}, a.model.kind, metric_form(a.metric), G, E, f);
+}
+cudaError_t launch_trajectory(const TrajArgs& a, cudaStream_t st, int* n_launches) {
+    return traj_dispatch(a, n_launches, [&](auto M, auto K, auto g, auto e) {
+        return launch_warps(trajectory_kernel<M, K, g, e>, a.N, g, smem_bytes(M, K, a.D, g), st, a);
+    });
 }
 cudaError_t launch_multinomial(const MultinomialArgs& a, cudaStream_t st, int* n_launches) {
-    int G, E;
-    if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
-    if (n_launches) *n_launches += 1;
-    AHMC_MM(mn_layout, a.model.kind, metric_form(a.metric));
+    return traj_dispatch(a, n_launches, [&](auto M, auto K, auto g, auto e) {
+        return launch_warps(multinomial_kernel<M, K, g, e>, a.N, g, smem_bytes(M, K, a.D, g), st, a);
+    });
 }
 
 #endif  // AHMC_SIMT_EMULATION

@@ -26,6 +26,9 @@
 // the Dense metric, WelfordCov (ahmc_nuts_cov.cu).
 #pragma once
 #include "ahmc_chain_adapt.cuh"
+#if !defined(AHMC_SIMT_EMULATION) && !defined(__CUDACC_RTC__)
+#include "ahmc_dispatch.cuh"
+#endif
 
 namespace ahmc {
 
@@ -39,9 +42,6 @@ __host__ __device__ inline long long nuts_level_doubles(int D, int max_depth) {
     return (long long)(9 + kLevelVecs * (max_depth > 0 ? max_depth : 1)) * D;
 }
 
-__device__ __forceinline__ double jl_min0(double x) {  // min(0, x), NaN-propagating like Julia
-    return (x != x) ? x : (x < 0.0 ? x : 0.0);
-}
 __device__ __forceinline__ double logaddexp(double a, double b) {  // LogExpFunctions.logaddexp
     double delta = (a == b) ? 0.0 : fabs(a - b);
     double mx = (a != a || b != b) ? CUDART_NAN : (a > b ? a : b);
@@ -247,7 +247,7 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
                 vload_nc<G, E>(s.th, first ? a.th_in + a.ld_in * chain : a.th_out + a.ld_out * chain, l, D);
                 vload_nc<G, E>(s.g, first ? a.g_in + a.ld_in * chain : a.g_out + a.ld_out * chain, l, D);
             }
-            if (a.refresh) {
+            if (a.refresh) {  // (written out, not draw_momentum: sharing it changes the variant family's generated code)
                 if (a.rng.normal_tape) {
                     vload_nc<G, E>(rn, a.rng.normal_tape + (long long)D * chain, l, D);
                 } else {
@@ -757,54 +757,17 @@ static cudaError_t launch_nuts_v(const NutsArgs& a, cudaStream_t st) {
         // dense operators, one chain per warp: blocks of kCoopWarps chains share every D x D product (COOP form)
         const long long blocks = (a.N + kCoopWarps - 1) / kCoopWarps;
         const size_t sm = ((size_t)coop_smem_doubles(a.D, coop_kc<E>()) + (size_t)kCoopWarps * maxd * kLevelScalars) * sizeof(double);
-        auto go = [&](auto kernel) -> cudaError_t {
-            if (sm > 48 * 1024) {
-                cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-                if (e != cudaSuccess) return e;
-            }
-            kernel<<<(unsigned)blocks, kCoopThreads, sm, st>>>(a);
-            return cudaGetLastError();
-        };
         if constexpr (E >= 2 && E <= 8) {
-            if (a.D == G * E) return go(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, true, true>);
+            if (a.D == G * E) return launch_kernel(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, true, true>, blocks, kCoopThreads, sm, st, a);
         }
-        return go(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, false, true>);
+        return launch_kernel(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, false, true>, blocks, kCoopThreads, sm, st, a);
     } else {
-        const int chains_per_block = kBlockThreads / G;
-        const long long blocks = (a.N + chains_per_block - 1) / chains_per_block;
-        size_t sm = smem_bytes(MODEL, METRIC, a.D, G) + (size_t)chains_per_block * maxd * kLevelScalars * sizeof(double);
+        const size_t sm = smem_bytes(MODEL, METRIC, a.D, G) + (size_t)(kBlockThreads / G) * maxd * kLevelScalars * sizeof(double);
         if constexpr (G == 32 && E >= 2 && E <= 8) {
-            if (a.D == G * E) {  // full tile: compile-time D
-                if (sm > 48 * 1024) {
-                    cudaError_t e = cudaFuncSetAttribute(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, true>,
-                                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-                    if (e != cudaSuccess) return e;
-                }
-                nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, true><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
-                return cudaGetLastError();
-            }
+            if (a.D == G * E) return launch_warps(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, true>, a.N, G, sm, st, a);  // full tile: compile-time D
         }
-        if (sm > 48 * 1024) {
-            cudaError_t e = cudaFuncSetAttribute(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, false>,
-                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-            if (e != cudaSuccess) return e;
-        }
-        nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, false><<<(unsigned)blocks, kBlockThreads, sm, st>>>(a);
-        return cudaGetLastError();
+        return launch_warps(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, false>, a.N, G, sm, st, a);
     }
-}
-
-template <int MODEL, int METRIC, bool VAR, int ADAPT>
-static cudaError_t nuts_layout(const NutsArgs& a, cudaStream_t st, int G, int E) {
-    if (G == 4 && E == 1) return launch_nuts_v<MODEL, METRIC, 4, 1, VAR, ADAPT>(a, st);
-    if (G == 8 && E == 1) return launch_nuts_v<MODEL, METRIC, 8, 1, VAR, ADAPT>(a, st);
-    if (G == 16 && E == 1) return launch_nuts_v<MODEL, METRIC, 16, 1, VAR, ADAPT>(a, st);
-    if (G == 32 && E == 1) return launch_nuts_v<MODEL, METRIC, 32, 1, VAR, ADAPT>(a, st);
-    if (G == 32 && E == 2) return launch_nuts_v<MODEL, METRIC, 32, 2, VAR, ADAPT>(a, st);
-    if (G == 32 && E == 4) return launch_nuts_v<MODEL, METRIC, 32, 4, VAR, ADAPT>(a, st);
-    if (G == 32 && E == 8) return launch_nuts_v<MODEL, METRIC, 32, 8, VAR, ADAPT>(a, st);
-    if (G == 32 && E == 16) return launch_nuts_v<MODEL, METRIC, 32, 16, VAR, ADAPT>(a, st);
-    return cudaErrorInvalidValue;
 }
 
 // model x metric dispatch of one (VAR, ADAPT) family (ADAPT: 0, or the adaptor's estimator form, ahmc_chain_adapt.cuh);
@@ -813,37 +776,17 @@ template <bool VAR, int ADAPT, bool ONE_METRIC>
 static cudaError_t nuts_dispatch(const NutsArgs& a, cudaStream_t st) {
     int G, E;
     if (!pick_layout(a.D, &G, &E)) return cudaErrorInvalidValue;
+    auto run = [&](auto metrics, int metric) {
+        return with_model_metric_layout(AllModels{}, metrics, a.model.kind, metric, G, E,
+                                        [&](auto M, auto K, auto g, auto e) { return launch_nuts_v<M, K, g, e, VAR, ADAPT>(a, st); });
+    };
     if constexpr (ONE_METRIC) {  // (compile-time: the family holds no kernels for the other metrics)
         // (WelfordCov: a Dense metric, shared or per chain, as the starting point; the launch reads the chain's own rows)
         constexpr int MK = ADAPT == AHMC_ADAPT_WELFORD_COV ? kMetricDenseChain : AHMC_METRIC_DIAG;
         if (a.metric.kind != (ADAPT == AHMC_ADAPT_WELFORD_COV ? AHMC_METRIC_DENSE : AHMC_METRIC_DIAG)) return cudaErrorInvalidValue;
-        switch (a.model.kind) {
-            case AHMC_MODEL_STD_NORMAL: return nuts_layout<AHMC_MODEL_STD_NORMAL, MK, VAR, ADAPT>(a, st, G, E);
-            case AHMC_MODEL_DIAG_GAUSS: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, MK, VAR, ADAPT>(a, st, G, E);
-            case AHMC_MODEL_DENSE_GAUSS: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, MK, VAR, ADAPT>(a, st, G, E);
-            case AHMC_MODEL_FUNNEL: return nuts_layout<AHMC_MODEL_FUNNEL, MK, VAR, ADAPT>(a, st, G, E);
-        }
-        return cudaErrorInvalidValue;
+        return run(Kinds<MK>{}, MK);
     } else {
-        switch (a.model.kind * 4 + metric_form(a.metric)) {
-            case 0: return nuts_layout<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
-            case 1: return nuts_layout<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
-            case 2: return nuts_layout<AHMC_MODEL_STD_NORMAL, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
-            case 3: return nuts_layout<AHMC_MODEL_STD_NORMAL, kMetricDenseChain, VAR, ADAPT>(a, st, G, E);
-            case 4: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
-            case 5: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
-            case 6: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
-            case 7: return nuts_layout<AHMC_MODEL_DIAG_GAUSS, kMetricDenseChain, VAR, ADAPT>(a, st, G, E);
-            case 8: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
-            case 9: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
-            case 10: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
-            case 11: return nuts_layout<AHMC_MODEL_DENSE_GAUSS, kMetricDenseChain, VAR, ADAPT>(a, st, G, E);
-            case 12: return nuts_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_UNIT, VAR, ADAPT>(a, st, G, E);
-            case 13: return nuts_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG, VAR, ADAPT>(a, st, G, E);
-            case 14: return nuts_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_DENSE, VAR, ADAPT>(a, st, G, E);
-            case 15: return nuts_layout<AHMC_MODEL_FUNNEL, kMetricDenseChain, VAR, ADAPT>(a, st, G, E);
-        }
-        return cudaErrorInvalidValue;
+        return run(AllMetrics{}, metric_form(a.metric));
     }
 }
 
