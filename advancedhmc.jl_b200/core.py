@@ -194,9 +194,16 @@ class Funnel(_Target):
 class UserTarget(_Target):
     """A user-supplied log pi / grad log pi as CUDA source, compiled at run time INTO the fused kernels
     (ahmc_model_create_user; the `h.dlp/dtheta` closure of src/hamiltonian.jl:45-48 as a device function).  `source` defines
-    `__device__ double ahmc_user_logp_grad(const double* theta, double* grad, int D, const double* params)` (PLUS gradient)
-    or, with `#define AHMC_USER_COORDWISE`, `__device__ double ahmc_user_coord(int d, double theta_d, const double* params,
-    double* grad_d)`.  Works with phasepoint, step, static HMC transitions, NUTS and find_good_stepsize_batched."""
+    one of three contracts, chosen by the source:
+      * `__device__ double ahmc_user_logp_grad(const double* theta, double* grad, int D, const double* params)` (PLUS
+        gradient), run by one lane of the chain's group;
+      * with `#define AHMC_USER_COORDWISE`, `__device__ double ahmc_user_coord(int d, double theta_d, const double* params,
+        double* grad_d)` for targets that are a sum over coordinates;
+      * with `#define AHMC_USER_GROUPWISE`, `__device__ double ahmc_user_logp_grad_group(const double* theta, double* grad,
+        int D, const double* params, ahmc_group g)`, run by all G lanes of the chain's group together (g.lane, g.size = G);
+        each grad[d] is written by one lane, the return value is the lane's share of log pi, and the group may use
+        `ahmc_group_sum(g, x)`, `ahmc_group_bcast(g, x, src)` and `ahmc_group_sync(g)`.
+    Works with phasepoint, step, static HMC transitions, NUTS and find_good_stepsize_batched."""
 
     def __init__(self, D: int, source: str, params=None, c0: float = 0.0):
         self.kind, self.D, self.c0 = L.MODEL_USER, int(D), float(c0)
@@ -216,7 +223,8 @@ class UserTarget(_Target):
 
     @staticmethod
     def check_source(source: str, D: int, kernel: int = 1, metric_kind: int = 1):
-        """compile-only check (no GPU needed): raises InvalidArgument with the NVRTC log if `source` does not compile"""
+        """compile-only check (no GPU needed) of a source in any of the three forms (one-lane, AHMC_USER_COORDWISE,
+        AHMC_USER_GROUPWISE): raises InvalidArgument with the NVRTC log if `source` does not compile"""
         log = C.create_string_buffer(8192)
         rc = L.load().ahmc_user_source_check(source.encode(), kernel, metric_kind, D, log, 8192)
         if rc != L.OK:

@@ -38,8 +38,24 @@ typedef unsigned long long uint64_t;
 //   __device__ double ahmc_user_coord(int d, double theta_d, const double* params, double* grad_d);      (and #define AHMC_USER_COORDWISE)
 //       for targets that are a sum over coordinates: the term of coordinate d and its derivative; every lane evaluates
 //       its own coordinates and the terms are summed by warp shuffles (as fast as the built-in diagonal targets).
+//   __device__ double ahmc_user_logp_grad_group(const double* theta, double* grad, int D, const double* params,
+//                                               ahmc_group g);                                      (and #define AHMC_USER_GROUPWISE)
+//       the general target evaluated by ALL G lanes of the chain's group together (g.lane in 0..G-1, g.size = G).  theta
+//       (read-only) and grad are the group's two shared-memory D-vectors; each grad[d] (PLUS gradient) is written by
+//       exactly one lane, whichever the user picks.  Returns the calling lane's share of log pi: the library sums the G
+//       shares in a fixed order (Grp::sum) and adds c0.  The library syncs the group before the call (theta staged) and
+//       after it (before the lanes read grad).  Inside, the group may use ahmc_group_sum / _bcast / _sync (defined at the
+//       end of this file).
+#if defined(AHMC_USER_COORDWISE) && defined(AHMC_USER_GROUPWISE)
+#error "the user target defines both AHMC_USER_COORDWISE and AHMC_USER_GROUPWISE: select one contract"
+#endif
+struct ahmc_group {
+    int lane;  // 0 .. size-1: this lane's index in the chain's group
+    int size;  // G in {4, 8, 16, 32}
+};
 __device__ double ahmc_user_logp_grad(const double* theta, double* grad, int D, const double* params);
 __device__ double ahmc_user_coord(int d, double theta_d, const double* params, double* grad_d);
+__device__ double ahmc_user_logp_grad_group(const double* theta, double* grad, int D, const double* params, ahmc_group g);
 #endif
 
 namespace ahmc {
@@ -736,7 +752,7 @@ struct ModelOps {
 
     // true: eval_part already returns the finished log pi on every lane (the model needs its own collective anyway);
     // false: it returns this lane's partial sum and log pi = finish(Grp::sum(partial)).
-#if defined(AHMC_NVRTC_USER_MODEL) && defined(AHMC_USER_COORDWISE)
+#if defined(AHMC_NVRTC_USER_MODEL) && (defined(AHMC_USER_COORDWISE) || defined(AHMC_USER_GROUPWISE))
     static constexpr bool kLpReduced = MODEL == AHMC_MODEL_FUNNEL;
 #else
     static constexpr bool kLpReduced = MODEL == AHMC_MODEL_FUNNEL || MODEL == AHMC_MODEL_USER;
@@ -785,6 +801,25 @@ struct ModelOps {
                 if (d < D) term = ahmc_user_coord(d, th[e], P, &gd);
                 g[e] = -gd;  // PhasePoint caches MINUS the gradient (hamiltonian.jl:45-48)
                 part += term;
+            }
+            return part;
+#elif defined(AHMC_USER_GROUPWISE)
+            // every call site reaches this with all lanes of the warp converged (the loops around it are steered by
+            // warp-wide votes), so the full-warp syncs below and the user's group collectives are well defined
+            double* gs = xs + D;
+            __syncwarp();
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                const int d = l + G * e;
+                if (d < D) xs[d] = th[e];
+            }
+            __syncwarp();
+            part = ahmc_user_logp_grad_group(xs, gs, D, P, ahmc_group{l, G});
+            __syncwarp();
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                const int d = l + G * e;
+                g[e] = (d < D) ? -gs[d] : 0.0;
             }
             return part;
 #else
@@ -1036,3 +1071,45 @@ __device__ __forceinline__ bool philox_bit(uint64_t seed, uint64_t offset, long 
 }
 
 }  // namespace ahmc
+
+#if defined(AHMC_NVRTC_USER_MODEL) && defined(AHMC_USER_GROUPWISE)
+// Collectives of the chain's group for ahmc_user_logp_grad_group (the user's source follows this file).  The G lanes of
+// the group call them together; they synchronise only those lanes, so groups sharing a warp may take different paths
+// through the user's code.  The sum is Grp::sum's xor butterfly (fixed order; every lane ends with identical bits).
+namespace ahmc {
+template <int G>
+__device__ __forceinline__ double user_group_sum(double v) {
+    unsigned m = FULL;
+    if constexpr (G < 32) m = Grp<G>::gmask();
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) v += __shfl_xor_sync(m, v, o);
+    return v;
+}
+}  // namespace ahmc
+__device__ __forceinline__ double ahmc_group_sum(ahmc_group g, double x) {
+    switch (g.size) {
+        case 4: return ahmc::user_group_sum<4>(x);
+        case 8: return ahmc::user_group_sum<8>(x);
+        case 16: return ahmc::user_group_sum<16>(x);
+        default: return ahmc::user_group_sum<32>(x);
+    }
+}
+// the value x of lane `src` (0..G-1) of the group
+__device__ __forceinline__ double ahmc_group_bcast(ahmc_group g, double x, int src) {
+    switch (g.size) {
+        case 4: return __shfl_sync(ahmc::Grp<4>::gmask(), x, src, 4);
+        case 8: return __shfl_sync(ahmc::Grp<8>::gmask(), x, src, 8);
+        case 16: return __shfl_sync(ahmc::Grp<16>::gmask(), x, src, 16);
+        default: return __shfl_sync(ahmc::FULL, x, src, 32);
+    }
+}
+// shared-memory writes of the group's lanes (to grad, say) become visible to the group
+__device__ __forceinline__ void ahmc_group_sync(ahmc_group g) {
+    switch (g.size) {
+        case 4: __syncwarp(ahmc::Grp<4>::gmask()); break;
+        case 8: __syncwarp(ahmc::Grp<8>::gmask()); break;
+        case 16: __syncwarp(ahmc::Grp<16>::gmask()); break;
+        default: __syncwarp(ahmc::FULL); break;
+    }
+}
+#endif

@@ -5,7 +5,9 @@
 // (NVRTC; the sources are embedded in the library at build time, ahmc_embedded_sources.cu) and the resulting kernels --
 // phasepoint, the fused trajectory (K1), the static transition (K2), NUTS (K3, default family), find_good_stepsize and the
 // adaptive forms of K2 and K3 (in-launch warm-up, ahmc_chain_adapt.cuh) -- are the same code as the built-in targets with ModelOps<AHMC_MODEL_USER>::eval calling the user's function.  One instantiation
-// (kernel x metric x layout) is compiled on first use and cached in the model.  NVRTC and the driver API are bound with
+// (kernel x metric x layout) is compiled on first use and cached in the model.  The source picks its contract
+// (ahmc_device.cuh): the one-lane function, AHMC_USER_COORDWISE or AHMC_USER_GROUPWISE; the translation unit defines the
+// macro the source names, so a source naming both meets the #error there.  NVRTC and the driver API are bound with
 // dlopen: the library loads without them and fails loudly (AHMC_ERR_UNSUPPORTED) when a user target is requested.
 #include <dlfcn.h>
 
@@ -162,6 +164,7 @@ static bool compile(UserModule* m, int which, int metric, int G, int E, int form
     // definitions follow
     std::string tu = "#define AHMC_NVRTC_USER_MODEL 1\n";
     if (m->src.find("AHMC_USER_COORDWISE") != std::string::npos) tu += "#define AHMC_USER_COORDWISE 1\n";
+    if (m->src.find("AHMC_USER_GROUPWISE") != std::string::npos) tu += "#define AHMC_USER_GROUPWISE 1\n";
     tu += std::string("#include \"") + unit + "\"\n#line 1 \"user_target.cu\"\n" + m->src + "\n";
     void* prog = nullptr;
     int rc = g_rtc.CreateProgram(&prog, tu.c_str(), "ahmc_user_tu.cu", kEmbeddedCount, kEmbeddedSources, kEmbeddedNames);

@@ -171,6 +171,14 @@ int ahmc_model_create_callback(ahmc_ctx* ctx, int32_t D, ahmc_logp_grad_fn fn, v
  *     #define AHMC_USER_COORDWISE
  *     __device__ double ahmc_user_coord(int d, double theta_d, const double* params, double* grad_d);
  *         for targets that are a sum over coordinates: term d and its derivative (every lane evaluates its own coordinates)
+ *     #define AHMC_USER_GROUPWISE
+ *     __device__ double ahmc_user_logp_grad_group(const double* theta, double* grad, int D, const double* params, ahmc_group g);
+ *         the general form run by ALL G lanes of the chain's group together (G = 4, 8, 16 or 32 by D; g.lane in 0..G-1,
+ *         g.size = G): theta (read-only) and grad are the shared-memory D-vectors of the first form, each grad[d] written by
+ *         exactly one lane of the user's choosing; the return value is the lane's SHARE of log pi (the library sums the
+ *         G shares in a fixed order).  The group may use ahmc_group_sum(g, x) (butterfly sum, identical bits on every
+ *         lane), ahmc_group_bcast(g, x, src) and ahmc_group_sync(g) (shared-memory writes visible to the group).  The
+ *         library syncs the group before the call and after it.  A source that selects both #define forms is refused.
  * It is compiled at run time (NVRTC, sm_90a) together with the library's own kernel sources on first use of each kernel, so
  * phasepoint, the fused trajectory, the static HMC transition, NUTS (MultinomialTS + GeneralisedNoUTurn) and
  * find_good_stepsize run on it exactly as on a built-in target: no host round trip per step.  params[n_params] (host) is
@@ -180,7 +188,8 @@ int ahmc_model_create_user(ahmc_ctx* ctx, int32_t D, const char* cuda_src, const
                            ahmc_model** out);
 /* Compile-only check of a user target (no device, no context needed): kernel 0 phasepoint, 1 trajectory, 2 static HMC,
  * 3 NUTS, 4 find_good_stepsize, 5 NUTS with in-launch adaptation (ahmc_nuts_adapt_sample_f64), 6 static HMC with in-launch
- * adaptation (ahmc_hmc_adapt_sample_f64); the layout follows from D.  AHMC_OK, or AHMC_ERR_INVALID with the NVRTC log in `log`. */
+ * adaptation (ahmc_hmc_adapt_sample_f64); the layout follows from D.  Any of the three forms above.  AHMC_OK, or
+ * AHMC_ERR_INVALID with the NVRTC log in `log`. */
 int ahmc_user_source_check(const char* cuda_src, int32_t kernel, int32_t metric_kind, int32_t D, char* log, int64_t log_len);
 int ahmc_model_destroy(ahmc_ctx* ctx, ahmc_model* model);
 

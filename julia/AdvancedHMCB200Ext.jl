@@ -171,8 +171,10 @@ end
 
 """
 User target as CUDA source compiled at run time INTO the fused kernels (ahmc_model_create_user): `src` defines
-`__device__ double ahmc_user_logp_grad(const double* theta, double* grad, int D, const double* params)` (or the
-coordinate-wise contract, see include/ahmc_b200.h).  Unlike a callback target it runs inside NUTS and costs no host round trip.
+`__device__ double ahmc_user_logp_grad(const double* theta, double* grad, int D, const double* params)`, or the
+coordinate-wise contract (`#define AHMC_USER_COORDWISE`), or the group contract (`#define AHMC_USER_GROUPWISE`,
+`ahmc_user_logp_grad_group(theta, grad, D, params, g)`, run by every lane of the chain's group, which returns its share of
+log π); see include/ahmc_b200.h.  Unlike a callback target it runs inside NUTS and costs no host round trip.
 """
 function B200Target(src::String, D::Integer; params::Vector{Float64}=Float64[], c0=0.0)
     out = Ref{Ptr{Cvoid}}(C_NULL)
