@@ -3,25 +3,34 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <chrono>
 #include <cstring>
 #include <new>
 #include <string>
 #include <vector>
 
-// defaults of the host-buffer lane (see leapfrog_host_pipelined): page-locked buffers are read and written by the kernel
-// directly in ONE launch whose residency is capped at one CTA per SM, so the grid runs in staggered waves and uploads
-// overlap downloads; pageable buffers go through the copy engines in two chunks.  The first calls of a shape measure the
-// candidate transports and keep the fastest.
-#define AHMC_PIPE_DIRECT_CHUNKS 1
-#define AHMC_PIPE_CE_CHUNKS 2
-#define AHMC_PIPE_DIRECT_OCC 1  // resident CTAs per SM of a direct-access launch (0 = no cap)
-
 #include "ahmc_chain_adapt.cuh"
 #include "ahmc_kernels.cuh"
 
 using namespace ahmc;
+
+// How the host-buffer lane (leapfrog_host_pipelined) moves a call's buffers.  A direct side has the kernel read or
+// write page-locked host memory itself; such a launch has its residency capped at one CTA per SM, so the grid runs in
+// staggered waves and uploads overlap downloads.  Otherwise that side goes through the copy engines.
+struct PipeTransport {
+    bool up_direct;    // the kernel loads theta / r / gradient / eps / Minv from host memory (else: copy-engine upload)
+    bool down_direct;  // the kernel stores its results to host memory (else: copy-engine download)
+    int chunks;        // pieces of the chain axis
+};
+// the autotune candidates, in the order they are tried
+constexpr PipeTransport kPipeCands[] = {{true, true, 1}, {false, false, 2}, {false, false, 4}, {false, true, 4}};
+constexpr int kPipeNCand = sizeof kPipeCands / sizeof kPipeCands[0];
+constexpr int kMaxPipeChunks = 4;  // the context keeps two events per chunk
+static_assert([] {
+    for (const PipeTransport& t : kPipeCands)
+        if (t.chunks > kMaxPipeChunks) return false;
+    return true;
+}(), "a candidate transport uses more chunks than kMaxPipeChunks");
 
 // a grow-only device buffer of the context (see ensure)
 struct DevBuf {
@@ -44,11 +53,10 @@ struct ahmc_ctx {
     DevBuf dense_ws;      // K4: padded Minv, norms, per-chain fallback mask
     DevBuf coop_ws;       // cooperative NUTS products: Minv and cholU with padded columns (coop_lds)
     DevBuf split_ws;      // callback (split-step) mode workspace
-    // host-buffer pipeline: H2D stream, compute stream (= stream), D2H stream, one event pair per chunk
-    static constexpr int kMaxPipeChunks = 32, kPipeStreams = 5;  // 3 upload, 1 download, 1 second compute
-    cudaStream_t pipe[kPipeStreams] = {};
-    cudaEvent_t ev_a = nullptr, ev_join[kPipeStreams] = {};
-    cudaEvent_t ev_in[kMaxPipeChunks][3] = {}, ev_k[kMaxPipeChunks] = {};
+    // host-buffer pipeline: upload stream, compute stream (= stream), download stream; per chunk an upload-done and a
+    // kernel-done event, and one event that joins the downloads back into the compute stream
+    cudaStream_t pipe[2] = {};  // upload, download
+    cudaEvent_t ev_a = nullptr, ev_down = nullptr, ev_in[kMaxPipeChunks] = {}, ev_k[kMaxPipeChunks] = {};
     // transport choice of the host-buffer lane, measured per problem shape on its first calls (leapfrog_host_pipelined)
     struct PipeTune {
         int64_t N;
@@ -56,7 +64,7 @@ struct ahmc_ctx {
         int key;       // has_g | has_dr << 1 | per-chain eps << 2 | per-chain Minv << 3
         int calls;     // trial calls made so far
         int chosen;    // -1 while measuring
-        double best_ms[8];
+        double best_ms[kPipeNCand];
     };
     std::vector<PipeTune> tune;
     std::string transport = "none";  // what the last host-buffer call used (ahmc_last_transport)
@@ -578,16 +586,14 @@ int ahmc_destroy(ahmc_ctx* ctx) {
     cudaFree(ctx->d_min_break);
     for (DevBuf* b : {&ctx->arena, &ctx->chain_ws, &ctx->summary_ws, &ctx->energy_ws, &ctx->dense_ws, &ctx->coop_ws, &ctx->split_ws})
         cudaFree(b->p);
-    for (int i = 0; i < ahmc_ctx::kPipeStreams; ++i) {
-        if (ctx->pipe[i]) cudaStreamDestroy(ctx->pipe[i]);
-        if (ctx->ev_join[i]) cudaEventDestroy(ctx->ev_join[i]);
-    }
-    for (int i = 0; i < ahmc_ctx::kMaxPipeChunks; ++i) {
-        for (int j = 0; j < 3; ++j)
-            if (ctx->ev_in[i][j]) cudaEventDestroy(ctx->ev_in[i][j]);
+    for (cudaStream_t s : ctx->pipe)
+        if (s) cudaStreamDestroy(s);
+    for (int i = 0; i < kMaxPipeChunks; ++i) {
+        if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
         if (ctx->ev_k[i]) cudaEventDestroy(ctx->ev_k[i]);
     }
     if (ctx->ev_a) cudaEventDestroy(ctx->ev_a);
+    if (ctx->ev_down) cudaEventDestroy(ctx->ev_down);
     if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
     return AHMC_OK;
@@ -815,11 +821,11 @@ static void* pinned_alias(const void* p) {
 
 static int pipe_resources(ahmc_ctx* ctx) {
     if (ctx->pipe[0]) return AHMC_OK;
-    for (int i = 0; i < ahmc_ctx::kPipeStreams; ++i) CU(cudaStreamCreateWithFlags(&ctx->pipe[i], cudaStreamNonBlocking));
+    for (cudaStream_t& s : ctx->pipe) CU(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
     CU(cudaEventCreateWithFlags(&ctx->ev_a, cudaEventDisableTiming));
-    for (int i = 0; i < ahmc_ctx::kPipeStreams; ++i) CU(cudaEventCreateWithFlags(&ctx->ev_join[i], cudaEventDisableTiming));
-    for (int i = 0; i < ahmc_ctx::kMaxPipeChunks; ++i) {
-        for (int j = 0; j < 3; ++j) CU(cudaEventCreateWithFlags(&ctx->ev_in[i][j], cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&ctx->ev_down, cudaEventDisableTiming));
+    for (int i = 0; i < kMaxPipeChunks; ++i) {
+        CU(cudaEventCreateWithFlags(&ctx->ev_in[i], cudaEventDisableTiming));
         CU(cudaEventCreateWithFlags(&ctx->ev_k[i], cudaEventDisableTiming));
     }
     return AHMC_OK;
@@ -829,12 +835,12 @@ static int pipe_resources(ahmc_ctx* ctx) {
 // sub-problem) that flow upload -> kernel -> download through separate streams linked chunk by chunk with events, so
 // the upload of chunk i+1 overlaps the kernel and the download of chunk i (PCIe is full duplex): the call costs about
 // max(H2D, D2H) + one chunk instead of their sum.  Same kernels, bit-identical results to the one-shot path.
-//   upload   : copy engines, theta / r / gradient on one stream or on one stream each (their fixed per-copy latencies
-//              overlap), or -- page-locked buffers only -- none at all: the kernel loads from host memory directly;
-//   download : copy engines on a third stream, or -- page-locked buffers only -- none: the kernel's stores go straight
+//   upload   : copy engines on one stream, or -- page-locked inputs only -- none at all: the kernel loads from host
+//              memory directly, in one chunk;
+//   download : copy engines on a second stream, or -- page-locked outputs only -- none: the kernel's stores go straight
 //              to host memory as posted PCIe writes.
-// Pageable buffers always take the copy-engine form.  Knobs for A/B measurements: AHMC_PIPE_CHUNKS (chunk count),
-// AHMC_PIPE_UP = ce1 | ce3 | direct, AHMC_PIPE_DOWN = ce | direct, AHMC_PIPE_TRACE=1 (event timeline on stderr).
+// Each side is direct exactly when all of its buffers are page-locked.  A copy-engine upload takes 2 chunks from 1024
+// chains on (1 below).  When every buffer is page-locked and N >= 1024 the transport is measured instead (kPipeCands).
 static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, int32_t D,
                                    int64_t N, double eps, const double* eps_chain, int32_t n_steps,
                                    double temper_alpha, const ahmc_phasepoint* z_in, const ahmc_phasepoint* z_out,
@@ -843,7 +849,6 @@ static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const
     auto since = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_enter).count(); };
     int rc = pipe_resources(ctx);
     if (rc) return rc;
-    const char* ev;
     const bool per_chain_minv = metric->kind == AHMC_METRIC_DIAG && metric->chain_stride != 0;
 
     // which buffers can the device address directly?
@@ -868,26 +873,16 @@ static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const
     uint32_t* b_st = (uint32_t*)alias(status, out_pinned);
     int32_t* b_sd = (int32_t*)alias(steps_done, out_pinned);
 
-    const double t_attr = since();
-    enum { UP_CE1, UP_CE3, UP_DIRECT };
     const bool has_g = z_in->lp_gradient != nullptr;
-    int up = in_pinned ? UP_DIRECT : UP_CE1;
-    bool down_direct = out_pinned;
-    int occ_cap = AHMC_PIPE_DIRECT_OCC;
-    int nchunk = 0;
+    PipeTransport tp{in_pinned, out_pinned, in_pinned ? 1 : N >= 1024 ? 2 : 1};
     // ---- transport choice.  Page-locked buffers can be moved in several ways whose ranking depends on the HOST
     // (SM-issued reads of system memory are at the mercy of the platform's read-completion latency, copy engines are
     // not), so the first calls of a given shape try each candidate in turn -- results are bit-identical in every mode,
-    // nothing extra is executed -- and the fastest is kept for the life of the context.  Candidates: {direct loads + direct stores, 1 CTA/SM}, {copy engines, 2 / 4 chunks},
-    // {copy-engine upload, direct stores, 4 chunks}.  The AHMC_PIPE_* variables pin the choice (A/B runs).
-    struct Cand { int up; bool down_direct; int chunks; int occ; };
-    static const Cand kCands[] = {{UP_DIRECT, true, 1, 1}, {UP_CE1, false, 2, 0}, {UP_CE1, false, 4, 0}, {UP_CE1, true, 4, 1}};
-    constexpr int kNCand = 4, kRounds = 3;  // round 0 warms every candidate up (arena growth, first-touch), rounds 1.. are timed
-    const bool pinned_env = getenv("AHMC_PIPE_UP") || getenv("AHMC_PIPE_DOWN") || getenv("AHMC_PIPE_CHUNKS") || getenv("AHMC_PIPE_OCC");
-    const bool tunable = in_pinned && out_pinned && !pinned_env && N >= 1024 && !((ev = getenv("AHMC_PIPE_AUTOTUNE")) && atoi(ev) == 0);
+    // nothing extra is executed -- and the fastest is kept for the life of the context.
+    constexpr int kRounds = 3;  // round 0 warms every candidate up (arena growth, first-touch), rounds 1.. are timed
     ahmc_ctx::PipeTune* tune = nullptr;
     int trial = -1;
-    if (tunable) {
+    if (in_pinned && out_pinned && N >= 1024) {
         const int key = (has_g ? 1 : 0) | (z_out->lk_gradient ? 2 : 0) | (eps_chain ? 4 : 0) | (per_chain_minv ? 8 : 0);
         for (auto& t : ctx->tune)
             if (t.N == N && t.D == D && t.key == key) tune = &t;
@@ -900,34 +895,20 @@ static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const
         }
         int c = tune->chosen;
         if (c < 0) {
-            trial = tune->calls % kNCand;
+            trial = tune->calls % kPipeNCand;
             c = trial;
         }
-        up = kCands[c].up; down_direct = kCands[c].down_direct; nchunk = kCands[c].chunks; occ_cap = kCands[c].occ;
+        tp = kPipeCands[c];
     }
-    if ((ev = getenv("AHMC_PIPE_UP"))) up = !strcmp(ev, "direct") ? UP_DIRECT : !strcmp(ev, "ce3") ? UP_CE3 : UP_CE1;
-    if ((ev = getenv("AHMC_PIPE_DOWN"))) down_direct = !strcmp(ev, "direct");
-    if (!in_pinned && up == UP_DIRECT) up = UP_CE3;
-    if (!out_pinned) down_direct = false;
-    const bool trace = (ev = getenv("AHMC_PIPE_TRACE")) && atoi(ev) != 0;
-    if ((ev = getenv("AHMC_PIPE_OCC"))) occ_cap = atoi(ev);
-    if ((ev = getenv("AHMC_PIPE_CHUNKS"))) nchunk = atoi(ev);
-    if (nchunk <= 0) {
-        if (up == UP_DIRECT) {
-            nchunk = AHMC_PIPE_DIRECT_CHUNKS;
-        } else {
-            nchunk = N >= 1024 ? AHMC_PIPE_CE_CHUNKS : 1;
-        }
-        if (nchunk < 1) nchunk = 1;
-    }
-    if (nchunk > ahmc_ctx::kMaxPipeChunks) nchunk = ahmc_ctx::kMaxPipeChunks;
-    int64_t chunk = (N + nchunk - 1) / nchunk;
+    int64_t chunk = (N + tp.chunks - 1) / tp.chunks;
     chunk = (chunk + 3) & ~(int64_t)3;
 
     // device staging for whatever is not addressed directly
     const int64_t ldi = z_in->ld, ldo = z_out->ld;
     const size_t nMinv = metric_minv_count(metric, D, N);
-    const bool stage_in = up != UP_DIRECT, stage_out = !down_direct;
+    const bool stage_in = !tp.up_direct, stage_out = !tp.down_direct;
+    // a launch that reads or writes host memory directly is capped at one resident CTA per SM (see PipeTransport)
+    const int occ_cap = tp.up_direct || tp.down_direct ? 1 : 0;
     const bool hasU = metric->kind == AHMC_METRIC_DENSE && metric->cholU;
     double *dMinv, *dU, *dEps, *dTh, *dR, *dG, *oTh, *oR, *oG, *oDr, *oLp, *oLk;
     uint32_t* oSt;
@@ -954,50 +935,29 @@ static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const
     Carver arena{(char*)ctx->arena.p};
     layout(arena);
 
-    cudaStream_t s_cmp = ctx->stream;
-    cudaStream_t s_up[3] = {ctx->pipe[0], up == UP_CE3 ? ctx->pipe[1] : ctx->pipe[0], up == UP_CE3 ? ctx->pipe[2] : ctx->pipe[0]};
-    cudaStream_t s_down = ctx->pipe[3];
-    const int n_up = up == UP_CE3 ? 3 : 1;
+    cudaStream_t s_cmp = ctx->stream, s_up = ctx->pipe[0], s_down = ctx->pipe[1];
 
     // everything is ordered after earlier work on the context stream; shared parameters (re-read by every chain, so
     // always staged) go first on the compute stream itself
     CU(cudaEventRecord(ctx->ev_a, s_cmp));
-    if (stage_in)
-        for (int j = 0; j < n_up; ++j) CU(cudaStreamWaitEvent(s_up[j], ctx->ev_a, 0));
+    if (stage_in) CU(cudaStreamWaitEvent(s_up, ctx->ev_a, 0));
     if (nMinv && !per_chain_minv) CU(cudaMemcpyAsync(dMinv, metric->Minv, nMinv * 8, cudaMemcpyHostToDevice, s_cmp));
     if (hasU) CU(cudaMemcpyAsync(dU, metric->cholU, (size_t)D * D * 8, cudaMemcpyHostToDevice, s_cmp));
-    if (!stage_in) {  // the second compute stream starts after the shared parameters have landed
-        CU(cudaEventRecord(ctx->ev_join[0], s_cmp));
-        CU(cudaStreamWaitEvent(ctx->pipe[4], ctx->ev_join[0], 0));
-    }
-
-    std::vector<cudaEvent_t> tr;  // optional timeline (timing events are created only when tracing)
-    auto mark = [&](cudaStream_t st) {
-        if (!trace) return;
-        cudaEvent_t e;
-        cudaEventCreate(&e);
-        cudaEventRecord(e, st);
-        tr.push_back(e);
-    };
-    mark(s_cmp);
 
     const int n_abs = n_steps < 0 ? -n_steps : n_steps;
     int nl = 0, k = 0;
     for (int64_t c0 = 0; c0 < N; c0 += chunk, ++k) {
         const int64_t n = (c0 + chunk <= N) ? chunk : N - c0;
         if (stage_in) {
-            CU(cudaMemcpyAsync(dTh + ldi * c0, z_in->theta + ldi * c0, (size_t)ldi * n * 8, cudaMemcpyHostToDevice, s_up[0]));
-            if (eps_chain) CU(cudaMemcpyAsync(dEps + c0, eps_chain + c0, (size_t)n * 8, cudaMemcpyHostToDevice, s_up[0]));
-            CU(cudaMemcpyAsync(dR + ldi * c0, z_in->r + ldi * c0, (size_t)ldi * n * 8, cudaMemcpyHostToDevice, s_up[1]));
+            CU(cudaMemcpyAsync(dTh + ldi * c0, z_in->theta + ldi * c0, (size_t)ldi * n * 8, cudaMemcpyHostToDevice, s_up));
+            if (eps_chain) CU(cudaMemcpyAsync(dEps + c0, eps_chain + c0, (size_t)n * 8, cudaMemcpyHostToDevice, s_up));
+            CU(cudaMemcpyAsync(dR + ldi * c0, z_in->r + ldi * c0, (size_t)ldi * n * 8, cudaMemcpyHostToDevice, s_up));
             if (per_chain_minv)
                 CU(cudaMemcpyAsync(dMinv + metric->chain_stride * c0, metric->Minv + metric->chain_stride * c0,
-                                   (size_t)metric->chain_stride * n * 8, cudaMemcpyHostToDevice, s_up[1]));
-            if (has_g) CU(cudaMemcpyAsync(dG + ldi * c0, z_in->lp_gradient + ldi * c0, (size_t)ldi * n * 8, cudaMemcpyHostToDevice, s_up[2]));
-            for (int j = 0; j < n_up; ++j) {
-                CU(cudaEventRecord(ctx->ev_in[k][j], s_up[j]));
-                CU(cudaStreamWaitEvent(s_cmp, ctx->ev_in[k][j], 0));
-            }
-            mark(s_up[n_up - 1]);
+                                   (size_t)metric->chain_stride * n * 8, cudaMemcpyHostToDevice, s_up));
+            if (has_g) CU(cudaMemcpyAsync(dG + ldi * c0, z_in->lp_gradient + ldi * c0, (size_t)ldi * n * 8, cudaMemcpyHostToDevice, s_up));
+            CU(cudaEventRecord(ctx->ev_in[k], s_up));
+            CU(cudaStreamWaitEvent(s_cmp, ctx->ev_in[k], 0));
         }
         LeapfrogArgs a{};
         a.model = model_dev(model);
@@ -1026,19 +986,15 @@ static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const
         a.status = !status ? nullptr : (stage_out ? oSt : b_st) + c0;
         a.steps_done = !steps_done ? nullptr : (stage_out ? oSd : b_sd) + c0;
         a.flags = flags;
-        a.resident_blocks_per_sm = (!stage_in || !stage_out) ? occ_cap : 0;
-        // with direct loads the kernels of different chunks may run side by side: alternate two streams
-        cudaStream_t s_k = (!stage_in && (k & 1)) ? ctx->pipe[4] : s_cmp;
-        CU(launch_leapfrog(a, s_k, &nl));
-        mark(s_k);
+        a.resident_blocks_per_sm = occ_cap;
+        CU(launch_leapfrog(a, s_cmp, &nl));
         if (stage_out) {
-            CU(cudaEventRecord(ctx->ev_k[k], s_k));
+            CU(cudaEventRecord(ctx->ev_k[k], s_cmp));
             CU(cudaStreamWaitEvent(s_down, ctx->ev_k[k], 0));
             CU(cudaMemcpyAsync(z_out->theta + ldo * c0, a.th_out, (size_t)ldo * n * 8, cudaMemcpyDeviceToHost, s_down));
             CU(cudaMemcpyAsync(z_out->r + ldo * c0, a.r_out, (size_t)ldo * n * 8, cudaMemcpyDeviceToHost, s_down));
             CU(cudaMemcpyAsync(z_out->lp_gradient + ldo * c0, a.g_out, (size_t)ldo * n * 8, cudaMemcpyDeviceToHost, s_down));
             if (a.dr_out) CU(cudaMemcpyAsync(z_out->lk_gradient + ldo * c0, a.dr_out, (size_t)ldo * n * 8, cudaMemcpyDeviceToHost, s_down));
-            mark(s_down);
         }
     }
     ctx->launches += nl;
@@ -1048,51 +1004,26 @@ static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const
         CU(cudaMemcpyAsync(z_out->lk_value, oLk, (size_t)N * 8, cudaMemcpyDeviceToHost, s_down));
         if (status) CU(cudaMemcpyAsync(status, oSt, (size_t)N * 4, cudaMemcpyDeviceToHost, s_down));
         if (steps_done) CU(cudaMemcpyAsync(steps_done, oSd, (size_t)N * 4, cudaMemcpyDeviceToHost, s_down));
-        mark(s_down);
-        CU(cudaEventRecord(ctx->ev_join[3], s_down));
-        CU(cudaStreamWaitEvent(s_cmp, ctx->ev_join[3], 0));
-    }
-    if (!stage_in && k > 1) {
-        CU(cudaEventRecord(ctx->ev_join[4], ctx->pipe[4]));
-        CU(cudaStreamWaitEvent(s_cmp, ctx->ev_join[4], 0));
+        CU(cudaEventRecord(ctx->ev_down, s_down));
+        CU(cudaStreamWaitEvent(s_cmp, ctx->ev_down, 0));
     }
     // host buffers are valid once everything joined into the context stream has retired
-    const double t_issued = since();
     CU(cudaStreamSynchronize(s_cmp));
     {
         char buf[96];
-        snprintf(buf, sizeof buf, "up=%s down=%s chunks=%d%s%s", up == UP_DIRECT ? "direct" : up == UP_CE3 ? "ce3" : "ce1",
-                 down_direct ? "direct" : "ce", k, (!stage_in || !stage_out) && occ_cap > 0 ? " occ=1" : "",
-                 tune ? (tune->chosen >= 0 ? " (autotuned)" : " (autotune trial)") : "");
+        snprintf(buf, sizeof buf, "up=%s down=%s chunks=%d%s%s", tp.up_direct ? "direct" : "ce1", tp.down_direct ? "direct" : "ce",
+                 k, occ_cap ? " occ=1" : "", tune ? (tune->chosen >= 0 ? " (autotuned)" : " (autotune trial)") : "");
         ctx->transport = buf;
     }
     if (tune && trial >= 0) {
         const double ms = since();
-        if (tune->calls >= kNCand && ms < tune->best_ms[trial]) tune->best_ms[trial] = ms;
-        if (++tune->calls >= kNCand * kRounds) {
+        if (tune->calls >= kPipeNCand && ms < tune->best_ms[trial]) tune->best_ms[trial] = ms;
+        if (++tune->calls >= kPipeNCand * kRounds) {
             int best = 0;
-            for (int c = 1; c < kNCand; ++c)
+            for (int c = 1; c < kPipeNCand; ++c)
                 if (tune->best_ms[c] < tune->best_ms[best]) best = c;
             tune->chosen = best;
-            if (trace)
-                fprintf(stderr, "[ahmc pipe] autotune N=%lld D=%d: %.3f %.3f %.3f %.3f ms -> candidate %d\n", (long long)N, D,
-                        tune->best_ms[0], tune->best_ms[1], tune->best_ms[2], tune->best_ms[3], best);
         }
-    }
-    if (trace)
-        fprintf(stderr, "[ahmc pipe] host ms: pointer queries %.3f, everything issued %.3f, synchronised %.3f\n", t_attr,
-                t_issued, since());
-    if (trace && !tr.empty()) {
-        fprintf(stderr, "[ahmc pipe] up=%s down=%s chunks=%d x %lld chains; ms after the first mark, per chunk [upload] kernel [download]:\n ",
-                up == UP_DIRECT ? "direct" : up == UP_CE3 ? "ce3" : "ce1", down_direct ? "direct" : "ce", k, (long long)chunk);
-        const int per = 1 + (stage_in ? 1 : 0) + (stage_out ? 1 : 0);
-        for (size_t i = 1; i < tr.size(); ++i) {
-            float ms = 0.f;
-            cudaEventElapsedTime(&ms, tr[0], tr[i]);
-            fprintf(stderr, "%s%.3f", (i - 1) % per == 0 ? " | " : " ", ms);
-        }
-        fprintf(stderr, "\n");
-        for (cudaEvent_t e : tr) cudaEventDestroy(e);
     }
     return AHMC_OK;
 }

@@ -599,30 +599,38 @@ def test_nuts_sampling_moments_philox():
     assert tr.stat["acceptance_rate"].mean().item() > 0.6
 
 
-@pytest.mark.parametrize("pinned", [False, True])
-@pytest.mark.parametrize("up,down,chunks", [("ce1", "ce", "0"), ("ce3", "ce", "5"), ("ce3", "direct", "0"),
-                                            ("direct", "direct", "3"), ("direct", "ce", "2"), (None, None, None)])
-def test_pipelined_host_path_equals_device_path(up, down, chunks, pinned, monkeypatch):
-    """host-buffer calls with N >= 256 take the chunked upload / kernel / download lane: same bytes out as the device
-    call for every transport (copy engines on one or three streams, direct loads / stores on page-locked buffers,
-    ragged chunk counts, library defaults), with pageable and with page-locked arrays."""
-    if up is not None:
-        monkeypatch.setenv("AHMC_PIPE_UP", up)
-        monkeypatch.setenv("AHMC_PIPE_DOWN", down)
-        monkeypatch.setenv("AHMC_PIPE_CHUNKS", chunks)
-    D, N = 100, 4099
+@pytest.mark.parametrize("out_pinned", [False, True])
+@pytest.mark.parametrize("in_pinned", [False, True])
+@pytest.mark.parametrize("N", [300, 1023, 1024, 4099])
+def test_pipelined_host_path_equals_device_path(N, in_pinned, out_pinned):
+    """host-buffer calls with N >= 256 take the chunked upload / kernel / download lane.  Each side is moved by the kernel
+    itself when all of its buffers are page-locked and by the copy engines otherwise; a copy-engine upload is cut in 2
+    chunks from 1024 chains on (ragged at N = 4099); with everything page-locked from 1024 chains on, the first four
+    calls of a shape try the four candidate transports.  Every call returns the same bytes as the device call, and
+    ahmc_last_transport names the transport the residency selects."""
+    import ctypes as C
+
+    D = 100
     rng = np.random.default_rng(5)
     s = np.exp(rng.uniform(-1, 1, D))
     m = rng.normal(size=D)
     hold = []
 
-    def buf(a):
+    def buf(a, pinned):
         if not pinned:
             return np.ascontiguousarray(a)
         t = torch.as_tensor(np.ascontiguousarray(a)).pin_memory()
         hold.append(t)
         return t.numpy()
 
+    if in_pinned and out_pinned and N >= 1024:
+        want = ["up=direct down=direct chunks=1 occ=1 (autotune trial)", "up=ce1 down=ce chunks=2 (autotune trial)",
+                "up=ce1 down=ce chunks=4 (autotune trial)", "up=ce1 down=direct chunks=4 occ=1 (autotune trial)"]
+    else:
+        chunks = 1 if in_pinned or N < 1024 else 2
+        want = [f"up={'direct' if in_pinned else 'ce1'} down={'direct' if out_pinned else 'ce'} chunks={chunks}"
+                + (" occ=1" if in_pinned or out_pinned else "")]
+    ctx = A.get_context(0)
     Minv_pc = np.exp(rng.uniform(-1, 1, (N, D)))
     th, r = rng.normal(size=(N, D)), rng.normal(size=(N, D))
     eps = 0.05 * np.exp(rng.uniform(-0.3, 0.3, N))
@@ -630,17 +638,28 @@ def test_pipelined_host_path_equals_device_path(up, down, chunks, pinned, monkey
         hd = A.Hamiltonian(A.DiagEuclideanMetric(Minv), A.DiagGaussian(m, s))
         zd, infod = A.step(A.Leapfrog(torch.as_tensor(eps, device=DEV)), hd,
                            A.phasepoint(hd, torch.as_tensor(th, device=DEV), torch.as_tensor(r, device=DEV)), 17, return_info=True)
-        hh = A.Hamiltonian(A.DiagEuclideanMetric(buf(Minv)), A.DiagGaussian(m, s))
-        z0 = A.phasepoint(hh, buf(th), buf(r))
-        z0.lp.gradient = buf(z0.lp.gradient)
-        out = None
-        if pinned:
-            out = A.PhasePoint(buf(np.zeros((N, D))), buf(np.zeros((N, D))), A.DualValue(buf(np.zeros(N)), buf(np.zeros((N, D)))),
-                               A.DualValue(buf(np.zeros(N)), buf(np.zeros((N, D)))))
-        zh, infoh = A.step(A.Leapfrog(buf(eps)), hh, z0, 17, return_info=True, out=out)
-        for a, b in [(zh.theta, zd.theta), (zh.r, zd.r), (zh.lp.value, zd.lp.value), (zh.lk.value, zd.lk.value),
-                     (zh.lp.gradient, zd.lp.gradient), (zh.lk.gradient, zd.lk.gradient), (infoh.steps_done, infod.steps_done)]:
-            assert np.array_equal(a, b.cpu().numpy())
+        hh = A.Hamiltonian(A.DiagEuclideanMetric(buf(Minv, in_pinned)), A.DiagGaussian(m, s))
+        z0 = A.phasepoint(hh, buf(th, in_pinned), buf(r, in_pinned))
+        z0.lp.gradient = buf(z0.lp.gradient, in_pinned)
+        eh = buf(eps, in_pinned)
+        md, keep = hh.metric._desc(D, N, z0.theta)
+        zh = A.PhasePoint(*(buf(np.zeros((N, D)), out_pinned) for _ in range(2)),
+                          *(A.DualValue(buf(np.zeros(N), out_pinned), buf(np.zeros((N, D)), out_pinned)) for _ in range(2)))
+        status, steps_done = buf(np.zeros(N, np.int32), out_pinned), buf(np.zeros(N, np.int32), out_pinned)
+        zc, oc = z0._c(), zh._c()
+        seen = []
+        for _ in want:  # the raw ABI call: status and steps_done take the residency of the other outputs
+            for a in (zh.theta, zh.r, zh.lp.value, zh.lp.gradient, zh.lk.value, zh.lk.gradient, status, steps_done):
+                a[...] = 0
+            ctx.check(ctx.lib.ahmc_leapfrog_f64(ctx.h, hh.target.handle(ctx), C.byref(md), D, N, 0.0, eh.ctypes.data, 17, 0.0,
+                                                C.byref(zc), C.byref(oc), status.ctypes.data, steps_done.ctypes.data,
+                                                A.FLAG_HOST_BUFFERS))
+            seen.append(ctx.last_transport())
+            for a, b in [(zh.theta, zd.theta), (zh.r, zd.r), (zh.lp.value, zd.lp.value), (zh.lk.value, zd.lk.value),
+                         (zh.lp.gradient, zd.lp.gradient), (zh.lk.gradient, zd.lk.gradient), (status, infod.status),
+                         (steps_done, infod.steps_done)]:
+                assert np.array_equal(a, b.cpu().numpy()), seen[-1]
+        assert seen == want
 
 
 @pytest.mark.parametrize("model,metric,D,N", [("diag_gauss", "diag", 128, 300), ("diag_gauss", "diag", 100, 300), ("std_normal", "unit", 64, 77),
@@ -678,11 +697,9 @@ def test_step_without_cached_gradient_equals_step_with_it(model, metric, D, N):
         A.step(A.Leapfrog(0.07), h, A.PhasePoint(z0.theta, z0.r, A.DualValue(None, None), A.DualValue(None, None)), 0)
 
 
-def test_host_lane_autotune_tries_every_transport_and_stays_bit_identical(monkeypatch):
+def test_host_lane_autotune_tries_every_transport_and_stays_bit_identical():
     """page-locked buffers: the first 12 calls of a shape walk through the four transports (3 rounds), then the fastest is
     kept; every call returns the same bytes as the device call; ahmc_last_transport names what was used."""
-    for k in ("AHMC_PIPE_UP", "AHMC_PIPE_DOWN", "AHMC_PIPE_CHUNKS", "AHMC_PIPE_OCC", "AHMC_PIPE_AUTOTUNE"):
-        monkeypatch.delenv(k, raising=False)
     D, N = 128, 2051
     m, s, Minv, th, r = synth_diag_gauss(D, N, seed=9)
     h = A.Hamiltonian(A.DiagEuclideanMetric(Minv), A.DiagGaussian(m, s))
