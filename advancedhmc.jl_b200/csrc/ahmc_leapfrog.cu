@@ -95,12 +95,13 @@ struct StepIO {
     }
 };
 
-// Occupancy: 7 blocks of 4 warps per SM, i.e. <= 72 registers per thread.  On an H100 (132 SMs x 7 x 4 = 3696 warp
-// slots) the headline batch (4096 chains x D=128 -> 4096 warps) runs as one full wave plus a 10 % tail.  Capping at 8
-// blocks (64 registers) would make it one wave but spills inside the fast path, and measured slower (H100 SXM, 400 W
-// power limit, L2 flushed: 14.5 against 14.4 us per launch at 4096 chains, 40.4 against 37.5 us at 16384).  The cap
-// makes the (rarely taken) exact fallback of the separable kernels spill a little, which is the right trade.  Wider
-// layouts (E >= 8) and non-separable models keep the default budget.
+// Occupancy of the one-chain-per-group kernel: 7 blocks of 4 warps per SM, i.e. <= 72 registers per thread.  With one
+// chain per warp the headline batch (4096 chains x D=128) would be one full wave of 3696 warps plus a 10 % tail on an
+// H100; capping at 8 blocks (64 registers) made it one wave but measured no faster (H100 SXM, 400 W power limit, L2
+// flushed: 14.5 against 14.4 us per launch), since the load, compute and store phases of one wave do not overlap.  The
+// headline shape now runs leapfrog_pair_kernel (below: two chains per warp, 4 blocks per SM, one wave).  The cap makes
+// the (rarely taken) exact fallback of the separable kernels spill a little, which is the right trade.  Wider layouts
+// (E >= 8) and non-separable models keep the default budget.
 template <int MODEL, int METRIC, int E>
 constexpr int min_blocks_per_sm() {
     return (FastCapable<MODEL, METRIC>::value && E <= 4) ? 7 : 1;
@@ -133,6 +134,87 @@ __global__ void __launch_bounds__(kBlockThreads, min_blocks_lf<MODEL, METRIC, E>
     StepIO<G, E, CONTIG> io{a, chain, l};
     run_trajectory<MODEL, METRIC, G, E>(a.model, a.metric, a.D, chain, valid, l, xs, eps, a.n_steps, a.temper_alpha,
                                         a.flags, io);
+}
+
+// K1's fast path on lane-contiguous full tiles (D = 64, 128; launched only without tempering or exact checks): warp w
+// integrates TWO chains, A = 2w and B = 2w + 1, one after the other, and B's loads are issued only once A's state has
+// arrived and passed its magnitude test, so they are in flight while A integrates and stores.  With one chain per warp
+// every warp of the wave issues its loads at once, DRAM serves them interleaved, and the whole wave then computes with
+// HBM idle and stores at once.  Each chain goes through run_trajectory's fast-path arithmetic (FastCoef) op for op, so
+// the results are bit-identical to the one-chain kernel.  SHARED: scalar eps and a shared M^-1, so A's coefficient
+// registers serve B too (what keeps the pair within 128 registers at E = 4); otherwise B builds its own after A is done.
+// 4 blocks of 4 warps per SM (<= 128 registers): the headline 4096 chains are 2048 warps, one wave on 132 SMs.
+template <int MODEL, int METRIC, int E, bool SHARED>
+__global__ void __launch_bounds__(kBlockThreads, 4) leapfrog_pair_kernel(const LeapfrogArgs a) {
+    constexpr int G = 32;
+    extern __shared__ double smem[];
+    const int l = threadIdx.x % G;
+    const int w = threadIdx.x / G;
+    const long long cA0 = 2 * ((long long)blockIdx.x * (kBlockThreads / G) + w), cB0 = cA0 + 1;
+    const long long cA = cA0 < a.N ? cA0 : a.N - 1, cB = cB0 < a.N ? cB0 : a.N - 1;  // past N: shadow the last chain
+    const bool vA = cA0 < a.N && (!a.only_mask || a.only_mask[cA] != 0);
+    const bool vB = cB0 < a.N && (!a.only_mask || a.only_mask[cB] != 0);
+    const int D = a.D, n = a.n_steps;
+    double epsA = a.eps_chain ? __ldg(a.eps_chain + cA) : a.eps, epsB = a.eps_chain ? __ldg(a.eps_chain + cB) : a.eps;
+    epsA = a.fwd ? epsA : -epsA;  // integrator.jl:226
+    epsB = a.fwd ? epsB : -epsB;
+    StepIO<G, E, true> ioA{a, cA, l}, ioB{a, cB, l};
+    FastCoef<MODEL, METRIC, G, E, true> k;
+    const bool have_g = ioA.has_g();
+
+    double xA[E], rA[E];
+    {
+        double g0[E], mi[E];
+        ioA.init_c(xA, rA, g0);
+        if constexpr (METRIC == AHMC_METRIC_DIAG) cload<E>(mi, a.metric.Minv + a.metric.chain_stride * cA, l, D);
+        k.load_model(a.model, l, D);
+        k.make(mi, epsA, n, l, D);
+        k.enter(xA, rA, g0, have_g);
+    }
+    bool sA = k.bad | k.test(xA, rA);
+
+    // B's loads.  Left alone the compiler issues them together with A's at the top of the kernel.  Their address is made
+    // to depend on a vote over A's test, which reads every element of A's state, through a term that is zero at run time
+    // but not to the compiler (%laneid equals l, which it cannot prove): the loads leave once A's state has arrived.
+#ifdef AHMC_SIMT_EMULATION
+    const unsigned lane = threadIdx.x % 32;
+#else
+    unsigned lane;
+    asm("mov.u32 %0, %%laneid;" : "=r"(lane));
+#endif
+    const long long offB = a.ld_in * cB + (long long)(__any_sync(FULL, sA) & (lane ^ (unsigned)l));
+    double xB[E], rB[E], gB[E], miB[E];
+    cload<E>(xB, a.th_in + offB, l, D);
+    cload<E>(rB, a.r_in + offB, l, D);
+    cload<E>(gB, (a.g_in ? a.g_in : a.th_in) + offB, l, D);
+    if constexpr (METRIC == AHMC_METRIC_DIAG && !SHARED) cload<E>(miB, a.metric.Minv + a.metric.chain_stride * cB, l, D);
+
+    bool needA, needB;
+    {
+        sA |= k.steps(xA, rA, n);
+        double g[E], dr[E], lp, lk;
+        k.last(xA, rA, g, dr, lp, lk, a.model.c0, l, D);
+        sA = Grp<G>::any(sA);
+        needA = vA && sA;
+        if (vA && !sA) ioA.done_c(xA, rA, g, dr, lp, lk, true, n);
+    }
+    {
+        if constexpr (!SHARED) k.make(miB, epsB, n, l, D);
+        k.enter(xB, rB, gB, have_g);
+        bool sB = k.bad | k.test(xB, rB);
+        sB |= k.steps(xB, rB, n);
+        double g[E], dr[E], lp, lk;
+        k.last(xB, rB, g, dr, lp, lk, a.model.c0, l, D);
+        sB = Grp<G>::any(sB);
+        needB = vB && sB;
+        if (vB && !sB) ioB.done_c(xB, rB, g, dr, lp, lk, true, n);
+    }
+
+    // a chain that failed its proof is re-run alone by the exact path, A then B, each with the whole warp
+    if (!__any_sync(FULL, needA || needB)) return;
+    double* xs = smem + (size_t)w * slab_vectors<MODEL>() * D;
+    exact_trajectory<MODEL, METRIC, G, E>(a.model, a.metric, D, cA, needA, l, xs, epsA, n, a.temper_alpha, ioA);
+    exact_trajectory<MODEL, METRIC, G, E>(a.model, a.metric, D, cB, needB, l, xs, epsB, n, a.temper_alpha, ioB);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -549,9 +631,9 @@ static bool contig_ok(const LeapfrogArgs& a) {
     return true;
 }
 
-template <int MODEL, int METRIC, int G, int E, bool CONTIG>
-static cudaError_t launch_lf_c(const LeapfrogArgs& a, cudaStream_t st) {
-    size_t sm = smem_bytes(MODEL, METRIC, a.D, G);
+// dynamic shared memory of a K1 launch (the pair kernel's exact path uses one group's slab per warp, as G = 32 does)
+static size_t lf_smem(int model, int metric, int G, const LeapfrogArgs& a) {
+    size_t sm = smem_bytes(model, metric, a.D, G);
     const int occ = a.resident_blocks_per_sm;
     if (occ > 0) {
         // occupancy throttle (host-memory lanes): pad the dynamic shared memory so that only this many CTAs fit on
@@ -559,13 +641,28 @@ static cudaError_t launch_lf_c(const LeapfrogArgs& a, cudaStream_t st) {
         const size_t pad = (size_t)(227 * 1024) / (size_t)occ - 1024;
         if (pad > sm) sm = pad;
     }
-    return launch_warps(leapfrog_kernel<MODEL, METRIC, G, E, CONTIG>, a.N, G, sm, st, a);
+    return sm;
+}
+template <int MODEL, int METRIC, int G, int E, bool CONTIG>
+static cudaError_t launch_lf_c(const LeapfrogArgs& a, cudaStream_t st) {
+    return launch_warps(leapfrog_kernel<MODEL, METRIC, G, E, CONTIG>, a.N, G, lf_smem(MODEL, METRIC, G, a), st, a);
 }
 template <int MODEL, int METRIC, int G, int E>
 static cudaError_t launch_lf_t(const LeapfrogArgs& a, cudaStream_t st) {
     if constexpr (FastCapable<MODEL, METRIC>::value && G == 32 && E >= 2) {
-        if (!(a.flags & AHMC_FLAG_EXACT_CHECKS) && !(a.temper_alpha > 0.0) && contig_ok<E>(a))
-            return launch_lf_c<MODEL, METRIC, G, E, true>(a, st);
+        if (!(a.flags & AHMC_FLAG_EXACT_CHECKS) && !(a.temper_alpha > 0.0) && contig_ok<E>(a)) {
+            if constexpr (E <= 4) {
+                // the pair kernel: 2 chains per warp, 8 per block
+                const size_t sm = lf_smem(MODEL, METRIC, G, a);
+                const bool shared = !a.eps_chain && (METRIC != AHMC_METRIC_DIAG || a.metric.chain_stride == 0);
+                const long long blocks = (a.N + 2 * (kBlockThreads / G) - 1) / (2 * (kBlockThreads / G));
+                return shared ? launch_kernel(leapfrog_pair_kernel<MODEL, METRIC, E, true>, blocks, kBlockThreads, sm, st, a)
+                              : launch_kernel(leapfrog_pair_kernel<MODEL, METRIC, E, false>, blocks, kBlockThreads, sm, st, a);
+            } else {
+                // D = 256, 512: two chains' state and in-flight loads do not fit 128 registers; one chain per warp
+                return launch_lf_c<MODEL, METRIC, G, E, true>(a, st);
+            }
+        }
     }
     return launch_lf_c<MODEL, METRIC, G, E, false>(a, st);
 }

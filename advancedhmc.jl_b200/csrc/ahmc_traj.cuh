@@ -42,127 +42,134 @@ struct FastCapable {
                                   (METRIC == AHMC_METRIC_UNIT || METRIC == AHMC_METRIC_DIAG);
 };
 
-template <int MODEL, int METRIC, int G, int E, class F>
-__device__ __forceinline__ void run_trajectory(const ModelDev& model, const MetricDev& metric, int D,
-                                               long long chain, bool valid, int l, double* xs, double eps, int n,
-                                               double temper_alpha, uint32_t flags, F& f) {
-    bool need_exact = valid;
+// The fast path's constants: per coordinate a = eps*Minv, b = eps*w, the mean m and w itself, and the magnitude proof's
+// segment length and entry threshold.  One set serves every chain with the same eps and M^-1 (both chains of a K1 pair
+// when eps is a scalar and M^-1 is shared).  C: the lane layout of the state vectors (the coefficients follow it).
+template <int MODEL, int METRIC, int G, int E, bool C>
+struct FastCoef {
+    double ca[E], cb[E], mu[E], wi[E];
+    double he, inv_eps;
+    int cseg, tb;
+    bool bad;  // eps or the coefficients outside the proof's range: every chain using them goes to the exact path
 
-    if constexpr (FastCapable<MODEL, METRIC>::value) {
-        const bool fast_on = !(flags & AHMC_FLAG_EXACT_CHECKS) && !(temper_alpha > 0.0);
-        if (fast_on) {
-            constexpr bool C = F::kContig;  // lane layout of the state vectors (coefficients follow it)
-            constexpr int T200 = expo_bits(200), T100 = expo_bits(100), T50 = expo_bits(50);
-            double x[E], r[E], ca[E], cb[E], mu[E];
-            // |eps| must be in [2^-100, 2^50] for the proof below and for the 1/eps rescaling of the last step
-            const double inv_eps = 1.0 / eps;
-            bool suspicious = big_d(eps, T50) | big_d(inv_eps, T100);
-            const double he = 0.5 * eps;
-            unsigned amax = 0u, bmax = 0u;  // top 32 bits of max|a|, max|b| (monotone in the magnitude)
-            {
-                double g0[E], mi[E], wi[E];
-                if constexpr (C) f.init_c(x, r, g0);
-                else f.init(x, r, g0);
-                const bool have_g = f.has_g();
-                if constexpr (METRIC == AHMC_METRIC_DIAG) {
-                    if constexpr (F::kChainMinv) {
-#pragma unroll
-                        for (int e = 0; e < E; ++e) mi[e] = f.minv[e];
-                    } else {
-                        lload<C, G, E>(mi, metric.Minv + metric.chain_stride * chain, l, D);
-                    }
-                }
-                if constexpr (MODEL == AHMC_MODEL_DIAG_GAUSS) {
-                    lload<C, G, E>(wi, model.p1, l, D);
-                    lload<C, G, E>(mu, model.p0, l, D);
-                }
-#pragma unroll
-                for (int e = 0; e < E; ++e) {
-                    const bool in = lin<C, G, E>(l, e, D);
-                    if constexpr (METRIC != AHMC_METRIC_DIAG) mi[e] = in ? 1.0 : 0.0;
-                    if constexpr (MODEL != AHMC_MODEL_DIAG_GAUSS) {
-                        wi[e] = in ? 1.0 : 0.0;
-                        mu[e] = 0.0;
-                    }
-                    ca[e] = eps * mi[e];
-                    cb[e] = eps * wi[e];
-                    const unsigned ha = (unsigned)__double2hiint(ca[e]) & 0x7fffffffu;
-                    const unsigned hb = (unsigned)__double2hiint(cb[e]) & 0x7fffffffu;
-                    amax = ha > amax ? ha : amax;
-                    bmax = hb > bmax ? hb : bmax;
-                    x[e] = x[e] - mu[e];  // shifted coordinate
-                    // without a cached gradient it is recomputed exactly as ModelOps::eval does: (theta - m) * w
-                    const double ge = have_g ? g0[e] : ((MODEL == AHMC_MODEL_DIAG_GAUSS) ? x[e] * wi[e] : x[e]);
-                    r[e] = fma(-he, ge, r[e]);  // first half kick uses the CACHED gradient (integrator.jl:237)
-                }
-            }
-            amax = grp_umax<G>(amax);
-            bmax = grp_umax<G>(bmax);
-            suspicious |= (amax >= 0x7ff00000u) | (bmax >= 0x7ff00000u);  // Inf / NaN coefficients
-            // upper bounds of max|a|, max|b| rebuilt from their high words (+1 in the last place of the high word)
-            const double Amax = __hiloint2double((int)(amax + 1u), 0);
-            const double Bmax = __hiloint2double((int)(bmax + 1u), 0);
-            // K = (1+A)(1+B) bounds the per-step growth of max(|x|,|r|); log2(K) <= exponent(K) + 1 = ek
-            const double K = (1.0 + Amax) * (1.0 + Bmax);
-            int ek = ((__double2hiint(K) >> 20) & 0x7ff) - 1023 + 1;  // K >= 1: ek >= 1
-            if (ek > 100 || !(K >= 1.0)) suspicious = true;           // also catches NaN / Inf
-            ek = ek < 1 ? 1 : (ek > 100 ? 100 : ek);
-            // Segments of `cseg` steps, each entered only if max(|x|,|r|) < 2^tb with tb + cseg*ek <= 300: every
-            // intermediate phase point of the segment is then below 2^300 and finite, energies included.  When the whole
-            // trajectory fits one segment (n*ek <= 240: the entry threshold is still >= 2^60) the test on the loaded state
-            // is the only one; otherwise test against 2^200 every floor(100/ek) steps.
-            int cseg, tb;
-            if (n * ek <= 240) {
-                cseg = n;
-                tb = (1023 + 300 - n * ek) << 20;
-            } else {
-                cseg = 100 / ek;
-                tb = T200;
-            }
-            int left = n;  // steps still to take; the last one is the split (drift, gradient, half kick, energies) step
-            for (;;) {
-#pragma unroll
-                for (int e = 0; e < E; ++e) suspicious |= big_d(x[e], tb) | big_d(r[e], tb);
-                const bool last = left <= cseg;
-                const int m = last ? left - 1 : cseg;
-                for (int j = 0; j < m; ++j) {
-#pragma unroll
-                    for (int e = 0; e < E; ++e) {
-                        x[e] = fma(ca[e], r[e], x[e]);
-                        r[e] = fma(-cb[e], x[e], r[e]);
-                    }
-                }
-                if (last) break;
-                left -= m;
-            }
-            // last step: drift, gradient, half kick, energies.  g = x*w and dH/dr = Minv*r are recovered from the
-            // per-coordinate constants as (x*b)/eps and (r*a)/eps (one extra rounding, ~1e-16 relative)
-            double g[E], dr[E];
-            double lp_part = 0.0, lk_part = 0.0;
+    __device__ __forceinline__ void load_model(const ModelDev& model, int l, int D) {
+        if constexpr (MODEL == AHMC_MODEL_DIAG_GAUSS) {
+            lload<C, G, E>(wi, model.p1, l, D);
+            lload<C, G, E>(mu, model.p0, l, D);
+        } else {
 #pragma unroll
             for (int e = 0; e < E; ++e) {
-                x[e] = fma(ca[e], r[e], x[e]);
-                g[e] = (MODEL == AHMC_MODEL_DIAG_GAUSS) ? (x[e] * cb[e]) * inv_eps : (lin<C, G, E>(l, e, D) ? x[e] : 0.0);
-                r[e] = fma(-he, g[e], r[e]);
-                lp_part = fma(x[e], g[e], lp_part);
-                dr[e] = (METRIC == AHMC_METRIC_DIAG) ? (r[e] * ca[e]) * inv_eps : r[e];
-                lk_part = fma(r[e], dr[e], lk_part);
-                x[e] = x[e] + mu[e];  // back to theta
-            }
-            suspicious = Grp<G>::any(suspicious);
-            const double lp = fma(-0.5, Grp<G>::sum(lp_part), model.c0);
-            const double lk = -0.5 * Grp<G>::sum(lk_part);
-            need_exact = valid && suspicious;
-            if (valid && !suspicious) {  // finite by the magnitude proof
-                if constexpr (C) f.done_c(x, r, g, dr, lp, lk, true, n);
-                else f.done(x, r, g, dr, lp, lk, true, n);
+                wi[e] = lin<C, G, E>(l, e, D) ? 1.0 : 0.0;
+                mu[e] = 0.0;
             }
         }
     }
+    // mi: the chain's M^-1 (read for a Diag metric only); needs load_model first
+    __device__ __forceinline__ void make(const double (&mi)[E], double eps, int n, int l, int D) {
+        constexpr int T200 = expo_bits(200), T100 = expo_bits(100), T50 = expo_bits(50);
+        // |eps| must be in [2^-100, 2^50] for the proof below and for the 1/eps rescaling of the last step
+        inv_eps = 1.0 / eps;
+        bad = big_d(eps, T50) | big_d(inv_eps, T100);
+        he = 0.5 * eps;
+        unsigned amax = 0u, bmax = 0u;  // top 32 bits of max|a|, max|b| (monotone in the magnitude)
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            ca[e] = eps * ((METRIC == AHMC_METRIC_DIAG) ? mi[e] : (lin<C, G, E>(l, e, D) ? 1.0 : 0.0));
+            cb[e] = eps * wi[e];
+            const unsigned ha = (unsigned)__double2hiint(ca[e]) & 0x7fffffffu;
+            const unsigned hb = (unsigned)__double2hiint(cb[e]) & 0x7fffffffu;
+            amax = ha > amax ? ha : amax;
+            bmax = hb > bmax ? hb : bmax;
+        }
+        amax = grp_umax<G>(amax);
+        bmax = grp_umax<G>(bmax);
+        bad |= (amax >= 0x7ff00000u) | (bmax >= 0x7ff00000u);  // Inf / NaN coefficients
+        // upper bounds of max|a|, max|b| rebuilt from their high words (+1 in the last place of the high word)
+        const double Amax = __hiloint2double((int)(amax + 1u), 0);
+        const double Bmax = __hiloint2double((int)(bmax + 1u), 0);
+        // K = (1+A)(1+B) bounds the per-step growth of max(|x|,|r|); log2(K) <= exponent(K) + 1 = ek
+        const double K = (1.0 + Amax) * (1.0 + Bmax);
+        int ek = ((__double2hiint(K) >> 20) & 0x7ff) - 1023 + 1;  // K >= 1: ek >= 1
+        if (ek > 100 || !(K >= 1.0)) bad = true;                  // also catches NaN / Inf
+        ek = ek < 1 ? 1 : (ek > 100 ? 100 : ek);
+        // Segments of `cseg` steps, each entered only if max(|x|,|r|) < 2^tb with tb + cseg*ek <= 300: every
+        // intermediate phase point of the segment is then below 2^300 and finite, energies included.  When the whole
+        // trajectory fits one segment (n*ek <= 240: the entry threshold is still >= 2^60) the test on the loaded state
+        // is the only one; otherwise test against 2^200 every floor(100/ek) steps.
+        if (n * ek <= 240) {
+            cseg = n;
+            tb = (1023 + 300 - n * ek) << 20;
+        } else {
+            cseg = 100 / ek;
+            tb = T200;
+        }
+    }
+    // shifted coordinate x = theta - m and the first half kick, which uses the CACHED gradient (integrator.jl:237);
+    // without one it is recomputed exactly as ModelOps::eval does: (theta - m) * w
+    __device__ __forceinline__ void enter(double (&x)[E], double (&r)[E], const double (&g0)[E], bool have_g) const {
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            x[e] = x[e] - mu[e];
+            const double ge = have_g ? g0[e] : ((MODEL == AHMC_MODEL_DIAG_GAUSS) ? x[e] * wi[e] : x[e]);
+            r[e] = fma(-he, ge, r[e]);
+        }
+    }
+    // the first segment's entry test
+    __device__ __forceinline__ bool test(const double (&x)[E], const double (&r)[E]) const {
+        bool s = false;
+#pragma unroll
+        for (int e = 0; e < E; ++e) s |= big_d(x[e], tb) | big_d(r[e], tb);
+        return s;
+    }
+    // the first n - 1 steps (2 dependent DFMAs per coordinate), testing the entry of every later segment
+    __device__ __forceinline__ bool steps(double (&x)[E], double (&r)[E], int n) const {
+        bool s = false;
+        int left = n;  // steps still to take; the last one is the split (drift, gradient, half kick, energies) step
+        for (;;) {
+            const bool last = left <= cseg;
+            const int m = last ? left - 1 : cseg;
+            for (int j = 0; j < m; ++j) {
+#pragma unroll
+                for (int e = 0; e < E; ++e) {
+                    x[e] = fma(ca[e], r[e], x[e]);
+                    r[e] = fma(-cb[e], x[e], r[e]);
+                }
+            }
+            if (last) break;
+            left -= m;
+#pragma unroll
+            for (int e = 0; e < E; ++e) s |= big_d(x[e], tb) | big_d(r[e], tb);
+        }
+        return s;
+    }
+    // last step: drift, gradient, half kick, energies (x back to theta).  g = x*w and dH/dr = Minv*r are recovered from the
+    // per-coordinate constants as (x*b)/eps and (r*a)/eps (one extra rounding, ~1e-16 relative)
+    __device__ __forceinline__ void last(double (&x)[E], double (&r)[E], double (&g)[E], double (&dr)[E], double& lp,
+                                         double& lk, double c0, int l, int D) const {
+        double lp_part = 0.0, lk_part = 0.0;
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            x[e] = fma(ca[e], r[e], x[e]);
+            g[e] = (MODEL == AHMC_MODEL_DIAG_GAUSS) ? (x[e] * cb[e]) * inv_eps : (lin<C, G, E>(l, e, D) ? x[e] : 0.0);
+            r[e] = fma(-he, g[e], r[e]);
+            lp_part = fma(x[e], g[e], lp_part);
+            dr[e] = (METRIC == AHMC_METRIC_DIAG) ? (r[e] * ca[e]) * inv_eps : r[e];
+            lk_part = fma(r[e], dr[e], lk_part);
+            x[e] = x[e] + mu[e];
+        }
+        lp = fma(-0.5, Grp<G>::sum(lp_part), c0);
+        lk = -0.5 * Grp<G>::sum(lk_part);
+    }
+};
 
+// The exact path of a chain group: every model x metric, run only when some group of the warp needs it (need_exact: a
+// valid chain that is not already done).  Called by all lanes of the warp.
+template <int MODEL, int METRIC, int G, int E, class F>
+__device__ __forceinline__ void exact_trajectory(const ModelDev& model, const MetricDev& metric, int D, long long chain,
+                                                 bool need_exact, int l, double* xs, double eps, int n,
+                                                 double temper_alpha, F& f) {
     if (!__any_sync(FULL, need_exact)) return;
 
-    // ------------------------------------------------------------------ EXACT path
     ModelOps<MODEL, G, E> mo;
     MetricOps<METRIC, G, E> me;
     mo.load(model, l, D);
@@ -192,6 +199,49 @@ __device__ __forceinline__ void run_trajectory(const ModelDev& model, const Metr
         }
         if (!__any_sync(FULL, active)) break;
     }
+}
+
+template <int MODEL, int METRIC, int G, int E, class F>
+__device__ __forceinline__ void run_trajectory(const ModelDev& model, const MetricDev& metric, int D,
+                                               long long chain, bool valid, int l, double* xs, double eps, int n,
+                                               double temper_alpha, uint32_t flags, F& f) {
+    bool need_exact = valid;
+
+    if constexpr (FastCapable<MODEL, METRIC>::value) {
+        const bool fast_on = !(flags & AHMC_FLAG_EXACT_CHECKS) && !(temper_alpha > 0.0);
+        if (fast_on) {
+            constexpr bool C = F::kContig;
+            FastCoef<MODEL, METRIC, G, E, C> k;
+            double x[E], r[E];
+            {
+                double g0[E], mi[E];
+                if constexpr (C) f.init_c(x, r, g0);
+                else f.init(x, r, g0);
+                if constexpr (METRIC == AHMC_METRIC_DIAG) {
+                    if constexpr (F::kChainMinv) {
+#pragma unroll
+                        for (int e = 0; e < E; ++e) mi[e] = f.minv[e];
+                    } else {
+                        lload<C, G, E>(mi, metric.Minv + metric.chain_stride * chain, l, D);
+                    }
+                }
+                k.load_model(model, l, D);
+                k.make(mi, eps, n, l, D);
+                k.enter(x, r, g0, f.has_g());
+            }
+            bool suspicious = k.bad | k.test(x, r);
+            suspicious |= k.steps(x, r, n);
+            double g[E], dr[E], lp, lk;
+            k.last(x, r, g, dr, lp, lk, model.c0, l, D);
+            suspicious = Grp<G>::any(suspicious);
+            need_exact = valid && suspicious;
+            if (valid && !suspicious) {  // finite by the magnitude proof
+                if constexpr (C) f.done_c(x, r, g, dr, lp, lk, true, n);
+                else f.done(x, r, g, dr, lp, lk, true, n);
+            }
+        }
+    }
+    exact_trajectory<MODEL, METRIC, G, E>(model, metric, D, chain, need_exact, l, xs, eps, n, temper_alpha, f);
 }
 
 }  // namespace ahmc
