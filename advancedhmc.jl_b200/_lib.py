@@ -16,6 +16,7 @@ MODEL_STD_NORMAL, MODEL_DIAG_GAUSS, MODEL_DENSE_GAUSS, MODEL_FUNNEL, MODEL_CALLB
 FLAG_HOST_BUFFERS, FLAG_COMPAT_BREAK_ALL, FLAG_ASYNC, FLAG_EXACT_CHECKS, FLAG_NO_REFRESH = 1, 2, 4, 8, 16
 FLAG_NUTS_SLICE_TS, FLAG_NUTS_CLASSIC, FLAG_NUTS_STRICT = 32, 64, 128
 STATUS_NONFINITE = 1
+GLM_BERNOULLI_LOGIT, GLM_POISSON_LOG = 0, 1
 
 _dp = C.POINTER(C.c_double)
 _vp = C.c_void_p
@@ -71,6 +72,8 @@ PROTOTYPES = {
     "ahmc_model_create_callback": (C.c_int, [_vp, C.c_int32, LOGP_GRAD_FN, _vp, C.POINTER(_vp)]),
     "ahmc_model_create_user": (C.c_int, [_vp, C.c_int32, C.c_char_p, _dp, C.c_int32, C.c_double, C.POINTER(_vp)]),
     "ahmc_user_source_check": (C.c_int, [C.c_char_p, C.c_int32, C.c_int32, C.c_int32, C.c_char_p, C.c_int64]),
+    "ahmc_model_create_glm": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32, _dp, _dp, _dp, C.c_double, C.POINTER(_vp)]),
+    "ahmc_glm_source": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_char_p, C.c_int64]),
     "ahmc_model_destroy": (C.c_int, [_vp, _vp]),
     "ahmc_phasepoint_f64": (C.c_int, [_vp, _vp, C.POINTER(Metric), C.c_int32, C.c_int64, C.POINTER(PhasePoint),
                                       C.c_uint32]),

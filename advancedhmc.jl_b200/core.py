@@ -231,6 +231,47 @@ class UserTarget(_Target):
             raise L.InvalidArgument(rc, log.value.decode())
 
 
+class GLMTarget(_Target):
+    """Generalised linear model with a Gaussian prior (ahmc_model_create_glm):
+    log pi(theta) = c0 + sum_i l_i(x_i' theta) - sum_d prior_prec[d] theta_d^2 / 2, with `family` "bernoulli_logit"
+    (y in {0, 1}) or "poisson_log" (y in 0, 1, ...).  X is (n, D), an intercept is a column of ones; prior_prec is a
+    scalar, a D-vector or None (flat prior).  Device-buffer phasepoint / step / static transitions with a Unit or Diag
+    metric and D <= 256 run the chain-tile kernel; everything else runs as a run-time compiled target (UserTarget)."""
+
+    FAMILIES = {"bernoulli_logit": L.GLM_BERNOULLI_LOGIT, "poisson_log": L.GLM_POISSON_LOG}
+
+    def __init__(self, X, y, family: str = "bernoulli_logit", prior_prec=None, c0: float = 0.0):
+        if family not in self.FAMILIES:
+            raise L.InvalidArgument(L.ERR_INVALID, f"unknown GLM family {family!r}: one of {sorted(self.FAMILIES)}")
+        self.X = np.ascontiguousarray(X, dtype=np.float64)
+        self.y = np.ascontiguousarray(y, dtype=np.float64).reshape(-1)
+        if self.X.ndim != 2 or self.X.shape[0] != self.y.size:
+            raise L.InvalidArgument(L.ERR_INVALID, "X must be (n, D) and y of length n")
+        self.kind, self.D, self.c0 = L.MODEL_USER, int(self.X.shape[1]), float(c0)
+        self.family = family
+        self.prior_prec = None if prior_prec is None else np.ascontiguousarray(
+            np.broadcast_to(np.asarray(prior_prec, dtype=np.float64), (self.D,)))
+        self._handles = {}
+
+    def handle(self, ctx: "Context"):
+        h = self._handles.get(ctx.device)
+        if h is None:
+            h = C.c_void_p()
+            pp = self.prior_prec
+            ctx.check(ctx.lib.ahmc_model_create_glm(ctx.h, self.FAMILIES[self.family], self.D, self.y.size,
+                                                    self.X.ctypes.data_as(L._dp), self.y.ctypes.data_as(L._dp),
+                                                    None if pp is None else pp.ctypes.data_as(L._dp), self.c0, C.byref(h)))
+            self._handles[ctx.device] = h
+        return h
+
+    def source(self) -> str:
+        """the CUDA source (group form) this target runs as on the run-time compiled kernels"""
+        n = L.load().ahmc_glm_source(self.FAMILIES[self.family], self.D, self.y.size, None, 0)
+        buf = C.create_string_buffer(n + 1)
+        L.load().ahmc_glm_source(self.FAMILIES[self.family], self.D, self.y.size, buf, n + 1)
+        return buf.value.decode()
+
+
 class _RawCuda:
     """zero-copy view of a raw device pointer for torch (via __cuda_array_interface__)."""
 

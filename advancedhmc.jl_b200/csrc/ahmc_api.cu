@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "ahmc_chain_adapt.cuh"
+#include "ahmc_glm.cuh"
 #include "ahmc_kernels.cuh"
 
 using namespace ahmc;
@@ -53,6 +54,7 @@ struct ahmc_ctx {
     DevBuf dense_ws;      // K4: padded Minv, norms, per-chain fallback mask
     DevBuf coop_ws;       // cooperative NUTS products: Minv and cholU with padded columns (coop_lds)
     DevBuf split_ws;      // callback (split-step) mode workspace
+    DevBuf glm_ws;        // K6 transitions: -grad log pi of the start point
     // host-buffer pipeline: upload stream, compute stream (= stream), download stream; per chunk an upload-done and a
     // kernel-done event, and one event that joins the downloads back into the compute stream
     cudaStream_t pipe[2] = {};  // upload, download
@@ -82,6 +84,11 @@ struct ahmc_model {
     ahmc_logp_grad_fn fn = nullptr;
     void* user = nullptr;
     UserModule* rtc = nullptr;  // AHMC_MODEL_USER: run-time compiled kernels
+    // ahmc_model_create_glm: kind is AHMC_MODEL_USER (d_p0 = [prior_prec | X | y], the generated group-form source); the
+    // tile kernel (K6) reads prior_prec and y from there and X from the padded copy
+    int glm_family = -1;  // AHMC_GLM_*, -1: not a GLM target
+    int glm_n = 0;
+    double* d_glm_X = nullptr;  // glm_padded_doubles(D, n)
 };
 
 namespace {
@@ -528,6 +535,108 @@ static int unfused_transition(ahmc_ctx* ctx, const HmcArgs& h, int* nl, Trajecto
     CU(launch_mh_select(m, ctx->stream, nl));
     return AHMC_OK;
 }
+
+// can the chain-tile kernel (K6) run this call?  A GLM target, device buffers, a Unit or Diag metric (shared or per
+// chain), no EXACT_CHECKS, and a tile shape for (D, n)
+bool glm_tile_eligible(const ahmc_model* model, const MetricDev& metric, uint32_t flags) {
+    int RB, CB, nc, stages;
+    size_t sm;
+    return model->glm_family >= 0 && metric.kind != AHMC_METRIC_DENSE &&
+           !(flags & (AHMC_FLAG_EXACT_CHECKS | AHMC_FLAG_HOST_BUFFERS | AHMC_FLAG_COMPAT_BREAK_ALL)) &&
+           glm_tile_shape(model->D, model->glm_n, &RB, &CB, &nc, &stages, &sm);
+}
+// the model and metric half of K6's argument block
+GlmArgs glm_args(const ahmc_model* model, const MetricDev& metric, int64_t N) {
+    GlmArgs g{};
+    g.family = model->glm_family; g.D = model->D; g.n = model->glm_n; g.N = N;
+    g.Xp = model->d_glm_X; g.prec = model->d_p0; g.y = model->d_p0 + model->D + (size_t)model->glm_n * model->D;
+    g.c0 = model->c0;
+    g.Minv = metric.kind == AHMC_METRIC_DIAG ? metric.Minv : nullptr;
+    g.chain_stride = metric.chain_stride;
+    return g;
+}
+// K6 dispatch, as try_dense_trajectory: 1 if handled, 0 if the call is not eligible, < 0 on error.  `a`: DEVICE pointers.
+int try_glm_trajectory(ahmc_ctx* ctx, const ahmc_model* model, const LeapfrogArgs& a, int n_abs, double eps, double temper_alpha,
+                       int* nl) {
+    if (!glm_tile_eligible(model, a.metric, a.flags) || temper_alpha > 0.0) return 0;
+    GlmArgs g = glm_args(model, a.metric, a.N);
+    g.eps = eps; g.eps_chain = a.eps_chain; g.n_steps = n_abs; g.fwd = a.fwd;
+    g.th_in = a.th_in; g.r_in = a.r_in; g.g_in = a.g_in; g.ld_in = a.ld_in;
+    g.th_out = a.th_out; g.r_out = a.r_out; g.g_out = a.g_out; g.dr_out = a.dr_out;
+    g.lp_out = a.lp_out; g.lk_out = a.lk_out; g.ld_out = a.ld_out;
+    g.status = a.status; g.steps_done = a.steps_done;
+    CU(launch_glm_traj(g, ctx->stream, nl));
+    return 1;
+}
+int glm_start_workspace(ahmc_ctx* ctx, size_t bytes, double** out) {  // -grad log pi of a transition's start point
+    int rc = ensure(ctx, ctx->glm_ws, bytes, "the GLM start-point workspace");
+    *out = (double*)ctx->glm_ws.p;
+    return rc;
+}
+// Static transitions of a GLM target on the tile kernel: per transition refresh -> kinetic energy -> K6 in place on z_out
+// -> MH select, enqueued back to back without a host synchronisation; transition t draws at Philox offset offset + t,
+// starts from transition t - 1's z_out and writes row t of `draws` and of the statistics.  The start point of each
+// transition is kept in the split workspace (a rejection re-reads it), so z_out may alias z_in.
+int glm_transitions(ahmc_ctx* ctx, const ahmc_model* model, const HmcArgs& h, int* nl) {
+    const LeapfrogArgs& a = h.lf;
+    const int D = a.D;
+    const long long N = a.N;
+    SplitWork w;
+    int rc = split_workspace(ctx, D, N, D, &w);
+    if (rc) return rc;
+    double *th0 = w.cb_grad, *g0, *lp0 = w.cb_lp;  // start point: theta in cb_grad, -grad in glm_ws, lp in cb_lp
+    if ((rc = glm_start_workspace(ctx, (size_t)D * N * sizeof(double), &g0))) return rc;
+    auto cp = [&](double* dst, long long ldd, const double* src, long long lds) -> cudaError_t {
+        if (dst == src) return cudaSuccess;
+        return cudaMemcpy2DAsync(dst, (size_t)ldd * 8, src, (size_t)lds * 8, (size_t)D * 8, (size_t)N, cudaMemcpyDeviceToDevice,
+                                 ctx->stream);
+    };
+    for (int t = 0; t < h.n_transitions; ++t) {
+        const double* th = t ? a.th_out : a.th_in;
+        const double* gr = t ? a.g_out : a.g_in;
+        const double* rr = t ? a.r_out : a.r_in;
+        const long long ld = t ? a.ld_out : a.ld_in;
+        CU(cp(th0, D, th, ld));
+        CU(cp(g0, D, gr, ld));
+        CU(cudaMemcpyAsync(lp0, t ? a.lp_out : a.lp_in, (size_t)N * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+        RngDev rng = h.rng;
+        rng.offset += (uint64_t)t;
+        if (h.refresh) {
+            MomentumArgs ma{};
+            ma.metric = a.metric; ma.D = D; ma.N = N; ma.seed = rng.seed; ma.offset = rng.offset;
+            ma.normal_tape = rng.normal_tape; ma.r = w.r0; ma.ld = D;
+            CU(launch_rand_momentum(ma, ctx->stream, nl));
+        } else {
+            CU(cp(w.r0, D, rr, ld));
+        }
+        SplitArgs k0{};  // lk0 = neg kinetic energy of the refreshed momentum
+        k0.metric = a.metric; k0.D = D; k0.N = N; k0.fwd = 1; k0.mul = 1.0; k0.no_kick = 1;
+        k0.r = w.r0; k0.lk = w.lk0; k0.ld = D;
+        CU(launch_kick_energy(k0, ctx->stream, nl));
+        LeapfrogArgs lf = a;
+        lf.th_in = th0; lf.g_in = g0; lf.r_in = w.r0; lf.ld_in = D;
+        lf.status = nullptr; lf.steps_done = nullptr; lf.dr_out = nullptr;
+        if ((rc = try_glm_trajectory(ctx, model, lf, a.n_steps, a.eps, 0.0, nl)) < 0) return rc;
+        MhArgs m{};
+        m.D = D; m.N = N; m.n_steps = a.n_steps;
+        m.th0 = th0; m.g0 = g0; m.lp0 = lp0; m.ld0 = D;
+        m.r0 = w.r0; m.lk0 = w.lk0;
+        m.th = a.th_out; m.r = a.r_out; m.g = a.g_out; m.lp = a.lp_out; m.lk = a.lk_out; m.ld = a.ld_out;
+        m.rng = rng;
+        m.st = h.st;
+        const size_t so = (size_t)t * N;
+        if (m.st.n_steps) m.st.n_steps += so;
+        if (m.st.is_accept) m.st.is_accept += so;
+        if (m.st.acceptance_rate) m.st.acceptance_rate += so;
+        if (m.st.log_density) m.st.log_density += so;
+        if (m.st.hamiltonian_energy) m.st.hamiltonian_energy += so;
+        if (m.st.hamiltonian_energy_error) m.st.hamiltonian_energy_error += so;
+        if (m.st.numerical_error) m.st.numerical_error += so;
+        CU(launch_mh_select(m, ctx->stream, nl));
+        if (h.draws) CU(cp(h.draws + so * D, D, a.th_out, a.ld_out));
+    }
+    return AHMC_OK;
+}
 }  // namespace
 
 // =================================================================================================
@@ -584,7 +693,7 @@ int ahmc_destroy(ahmc_ctx* ctx) {
     DeviceGuard g(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     cudaFree(ctx->d_min_break);
-    for (DevBuf* b : {&ctx->arena, &ctx->chain_ws, &ctx->summary_ws, &ctx->energy_ws, &ctx->dense_ws, &ctx->coop_ws, &ctx->split_ws})
+    for (DevBuf* b : {&ctx->arena, &ctx->chain_ws, &ctx->summary_ws, &ctx->energy_ws, &ctx->dense_ws, &ctx->coop_ws, &ctx->split_ws, &ctx->glm_ws})
         cudaFree(b->p);
     for (cudaStream_t s : ctx->pipe)
         if (s) cudaStreamDestroy(s);
@@ -725,6 +834,68 @@ int ahmc_user_source_check(const char* cuda_src, int32_t kernel, int32_t metric_
     return rc == 0 ? AHMC_OK : (rc == -3 ? AHMC_ERR_UNSUPPORTED : AHMC_ERR_INVALID);
 }
 
+int64_t ahmc_glm_source(int32_t family, int32_t D, int32_t n, char* buf, int64_t len) {
+    const std::string s = glm_group_source(family, D, n);
+    if (buf && len > 0) snprintf(buf, (size_t)len, "%s", s.c_str());
+    return (int64_t)s.size();
+}
+
+int ahmc_model_create_glm(ahmc_ctx* ctx, int32_t family, int32_t D, int32_t n, const double* X, const double* y,
+                          const double* prior_prec, double c0, ahmc_model** out) {
+    if (!ctx || !out) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/out");
+    *out = nullptr;
+    if (family != AHMC_GLM_BERNOULLI_LOGIT && family != AHMC_GLM_POISSON_LOG)
+        return fail(ctx, AHMC_ERR_INVALID, "unknown GLM family %d", family);
+    if (n < 1 || D < 1 || D > 512) return fail(ctx, AHMC_ERR_INVALID, "a GLM target needs n >= 1 rows and D in 1..512 (got n=%d, D=%d)", n, D);
+    if (!X || !y) return fail(ctx, AHMC_ERR_INVALID, "X / y is NULL");
+    for (size_t i = 0; i < (size_t)n * D; ++i)
+        if (!std::isfinite(X[i])) return fail(ctx, AHMC_ERR_INVALID, "X[%zu, %zu] is not finite", i / D, i % D);
+    for (int d = 0; prior_prec && d < D; ++d)
+        if (!std::isfinite(prior_prec[d]) || prior_prec[d] < 0.0)
+            return fail(ctx, AHMC_ERR_INVALID, "prior_prec[%d] = %g: precisions are finite and >= 0", d, prior_prec[d]);
+    double lgam = 0.0;
+    for (int i = 0; i < n; ++i) {
+        if (!std::isfinite(y[i])) return fail(ctx, AHMC_ERR_INVALID, "y[%d] is not finite", i);
+        if (family == AHMC_GLM_BERNOULLI_LOGIT && y[i] != 0.0 && y[i] != 1.0)
+            return fail(ctx, AHMC_ERR_INVALID, "y[%d] = %g: a Bernoulli response is 0 or 1", i, y[i]);
+        if (family == AHMC_GLM_POISSON_LOG) {
+            if (y[i] < 0.0 || y[i] != std::floor(y[i]))
+                return fail(ctx, AHMC_ERR_INVALID, "y[%d] = %g: a Poisson response is a non-negative integer", i, y[i]);
+            lgam += std::lgamma(y[i] + 1.0);
+        }
+    }
+    DeviceGuard g(ctx->device);
+    ahmc_model* m = new (std::nothrow) ahmc_model();
+    if (!m) return fail(ctx, AHMC_ERR_NOMEM, "out of host memory");
+    m->kind = AHMC_MODEL_USER;
+    m->D = D;
+    m->c0 = c0 - lgam;
+    m->glm_family = family;
+    m->glm_n = n;
+    char why[256];
+    // without NVRTC the model still exists: calls that need the run-time compiled kernels fail at first use
+    m->rtc = user_module_create(glm_group_source(family, D, n).c_str(), why, sizeof why);
+    std::vector<double> params((size_t)D + (size_t)n * D + n, 0.0);
+    if (prior_prec) memcpy(params.data(), prior_prec, sizeof(double) * D);
+    memcpy(params.data() + D, X, sizeof(double) * (size_t)n * D);
+    memcpy(params.data() + D + (size_t)n * D, y, sizeof(double) * n);
+    const int lds = glm_lds(D);
+    std::vector<double> Xp(glm_padded_doubles(D, n), 0.0);
+    for (int i = 0; i < n; ++i) memcpy(Xp.data() + (size_t)i * lds, X + (size_t)i * D, sizeof(double) * D);
+    if (cudaMalloc((void**)&m->d_p0, params.size() * 8) != cudaSuccess || cudaMalloc((void**)&m->d_glm_X, Xp.size() * 8) != cudaSuccess) {
+        ahmc_model_destroy(ctx, m);
+        return fail(ctx, AHMC_ERR_NOMEM, "cudaMalloc for the GLM data failed");
+    }
+    cudaError_t e = cudaMemcpy(m->d_p0, params.data(), params.size() * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(m->d_glm_X, Xp.data(), Xp.size() * 8, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        ahmc_model_destroy(ctx, m);
+        return fail(ctx, AHMC_ERR_CUDA, "copying the GLM data failed: %s", cudaGetErrorString(e));
+    }
+    *out = m;
+    return AHMC_OK;
+}
+
 int ahmc_model_destroy(ahmc_ctx* ctx, ahmc_model* m) {
     if (!m) return AHMC_OK;
     if (ctx) {
@@ -733,6 +904,7 @@ int ahmc_model_destroy(ahmc_ctx* ctx, ahmc_model* m) {
         cudaFree(m->d_p1);
         cudaFree(m->d_p1_pad);
         cudaFree(m->d_p1_coop);
+        cudaFree(m->d_glm_X);
         if (m->rtc) {
             cudaStreamSynchronize(ctx->stream);
             user_module_destroy(m->rtc);
@@ -778,6 +950,11 @@ int ahmc_phasepoint_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metri
         sa.r = const_cast<double*>(a.r); sa.g = a.g; sa.lp = a.lp; sa.lk = a.lk; sa.dr = a.dr;
         sa.cb_lp = w.cb_lp; sa.cb_grad = w.cb_grad; sa.ld = z->ld;
         CU(launch_kick_energy(sa, ctx->stream, &nl));
+    } else if (glm_tile_eligible(model, a.metric, flags)) {  // one pass of the tile kernel over the input point
+        GlmArgs ga = glm_args(model, a.metric, N);
+        ga.fwd = 1; ga.th_in = a.th; ga.r_in = a.r; ga.ld_in = ga.ld_out = z->ld;
+        ga.g_out = a.g; ga.dr_out = a.dr; ga.lp_out = a.lp; ga.lk_out = a.lk;
+        CU(launch_glm_traj(ga, ctx->stream, &nl));
     } else {
         CU(launch_phasepoint(a, ctx->stream, &nl));
     }
@@ -1097,6 +1274,8 @@ int ahmc_leapfrog_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric*
         int nl2 = 0;
         rc = try_dense_trajectory(ctx, model, a, n_abs, eps, temper_alpha, compat, &nl2);
         if (rc < 0) return rc;
+        if (rc == 0) rc = try_glm_trajectory(ctx, model, a, n_abs, eps, temper_alpha, &nl2);
+        if (rc < 0) return rc;
         if (rc == 1) {
             ctx->launches += nl2;
             return finish_call(ctx, st, flags);
@@ -1408,6 +1587,11 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
             return try_dense_trajectory(ctx, model, t, n_steps, eps, 0.0, false, &nl);
         });
         if (rc) return rc;
+        ctx->launches += nl;
+        return finish_call(ctx, st, flags);
+    }
+    if (!cfg && h.rng.partial_alpha == 0.0 && !(h.rng.temper_alpha > 0.0) && glm_tile_eligible(model, a.metric, flags)) {
+        if ((rc = glm_transitions(ctx, model, h, &nl))) return rc;
         ctx->launches += nl;
         return finish_call(ctx, st, flags);
     }

@@ -214,7 +214,10 @@ static bool compile(UserModule* m, int which, int metric, int G, int E, int form
 
 cudaError_t user_launch(UserModule* m, int which, int metric_kind, int G, int E, const void* args, unsigned blocks, size_t smem,
                         cudaStream_t st, int form) {
-    if (!m) return cudaErrorInvalidValue;
+    if (!m) {  // a target created without NVRTC (ahmc_model_create_glm): the general form is unavailable
+        t_user_err = "run-time compilation is unavailable: libnvrtc or the driver library could not be bound (set AHMC_NVRTC_LIB)";
+        return cudaErrorInvalidValue;
+    }
     const long long key =
         (long long)which | ((long long)metric_kind << 4) | ((long long)G << 8) | ((long long)E << 16) | ((long long)form << 24);
     auto it = m->fns.find(key);

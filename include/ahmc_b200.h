@@ -191,6 +191,23 @@ int ahmc_model_create_user(ahmc_ctx* ctx, int32_t D, const char* cuda_src, const
  * adaptation (ahmc_hmc_adapt_sample_f64); the layout follows from D.  Any of the three forms above.  AHMC_OK, or
  * AHMC_ERR_INVALID with the NVRTC log in `log`. */
 int ahmc_user_source_check(const char* cuda_src, int32_t kernel, int32_t metric_kind, int32_t D, char* log, int64_t log_len);
+/* Generalised linear model with a Gaussian prior:
+ *     log pi(theta) = c0 + sum_i l_i(x_i' theta) - sum_d prior_prec[d] theta_d^2 / 2
+ * X: n x D row-major HOST array, y: n, prior_prec: D (NULL: flat prior); copied to the device at creation, together with
+ * the row-padded copy of X that the tile kernel streams.  The Poisson constant -sum_i lgamma(y_i + 1) is folded into c0.
+ * An intercept is a column of ones in X.  AHMC_ERR_INVALID: n < 1, D outside 1..512, non-finite X / y / prior_prec,
+ * negative prior_prec, Bernoulli y outside {0, 1}, Poisson y negative or not an integer.
+ * Device-buffer phasepoint, leapfrog and static HMC transitions (one or several, without in-launch adaptation) with a
+ * Unit or Diag metric and D <= 256 run the chain-tile kernel (design-matrix products on the fp64 tensor pipe); every other
+ * call runs the target as a run-time compiled one (see ahmc_model_create_user: same kernels, same refusals, needs NVRTC
+ * at first use -- creation succeeds without it). */
+#define AHMC_GLM_BERNOULLI_LOGIT 0 /* y in {0,1}:  l_i = y_i eta_i - softplus(eta_i),  mu = 1/(1+e^-eta) */
+#define AHMC_GLM_POISSON_LOG 1     /* y in 0,1,..: l_i = y_i eta_i - exp(eta_i) - lgamma(y_i+1), mu = exp(eta) */
+int ahmc_model_create_glm(ahmc_ctx* ctx, int32_t family, int32_t D, int32_t n, const double* X, const double* y,
+                          const double* prior_prec, double c0, ahmc_model** out);
+/* The CUDA source (group form, params = [prior_prec | X | y]) a GLM target runs as when it takes the run-time compiled
+ * kernels; for ahmc_user_source_check.  Returns the source's length (without the terminator); writes at most len bytes. */
+int64_t ahmc_glm_source(int32_t family, int32_t D, int32_t n, char* buf, int64_t len);
 int ahmc_model_destroy(ahmc_ctx* ctx, ahmc_model* model);
 
 /* ---- hot path -------------------------------------------------------------------------------- */

@@ -183,6 +183,29 @@ function B200Target(src::String, D::Integer; params::Vector{Float64}=Float64[], 
                                     context().h, D, src, isempty(params) ? C_NULL : pointer(params), length(params), c0, out))
     return B200Target(out[], D, nothing)
 end
+"""
+Generalised linear model with a Gaussian prior (ahmc_model_create_glm): `family` 0 = Bernoulli-logit, 1 = Poisson-log,
+`X` n × D (row `i` is `x_i`; copied row-major), `prior_prec` a D-vector or `nothing` (flat prior).  On the reference side
+this is `Hamiltonian(metric, ℓπ, ∂ℓπ∂θ)` with ℓπ(θ) = c0 + Σᵢ lᵢ(xᵢ'θ) − Σ_d prior_prec[d] θ_d²/2 and its gradient.
+Like the rest of this shim it has not been executed (no Julia on the build machines).
+"""
+function B200GLMTarget(X::Matrix{Float64}, y::Vector{Float64}; family::Integer=0, prior_prec=nothing, c0=0.0)
+    n, D = size(X)
+    Xr = collect(transpose(X))  # D × n column-major = n × D row-major
+    out = Ref{Ptr{Cvoid}}(C_NULL)
+    pp = prior_prec === nothing ? Float64[] : Vector{Float64}(prior_prec)
+    GC.@preserve Xr y pp check(ccall((:ahmc_model_create_glm, libahmc), Cint,
+                                      (Ptr{Cvoid}, Int32, Int32, Int32, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Float64, Ref{Ptr{Cvoid}}),
+                                      context().h, family, D, n, pointer(Xr), pointer(y), isempty(pp) ? C_NULL : pointer(pp), c0, out))
+    return B200Target(out[], D, nothing)
+end
+"the CUDA source a GLM target runs as on the run-time compiled kernels (ahmc_glm_source)"
+function b200_glm_source(family::Integer, D::Integer, n::Integer)
+    len = ccall((:ahmc_glm_source, libahmc), Int64, (Int32, Int32, Int32, Ptr{UInt8}, Int64), family, D, n, C_NULL, 0)
+    buf = zeros(UInt8, len + 1)
+    GC.@preserve buf ccall((:ahmc_glm_source, libahmc), Int64, (Int32, Int32, Int32, Ptr{UInt8}, Int64), family, D, n, pointer(buf), length(buf))
+    return unsafe_string(pointer(buf))
+end
 "compile-only check of a user target (no GPU needed); returns the NVRTC log (empty = compiles)"
 function b200_user_source_check(src::String, D::Integer; kernel::Integer=1, metric_kind::Integer=1)
     log = zeros(UInt8, 8192)
