@@ -203,7 +203,8 @@ class UserTarget(_Target):
         int D, const double* params, ahmc_group g)`, run by all G lanes of the chain's group together (g.lane, g.size = G);
         each grad[d] is written by one lane, the return value is the lane's share of log pi, and the group may use
         `ahmc_group_sum(g, x)`, `ahmc_group_bcast(g, x, src)` and `ahmc_group_sync(g)`.
-    Works with phasepoint, step, static HMC transitions, NUTS and find_good_stepsize_batched."""
+    Works with phasepoint, step, static HMC transitions, NUTS, find_good_stepsize_batched and the in-launch warm-ups
+    (nuts_adapt_sample / hmc_adapt_sample) with a Diag or a Dense metric."""
 
     def __init__(self, D: int, source: str, params=None, c0: float = 0.0):
         self.kind, self.D, self.c0 = L.MODEL_USER, int(D), float(c0)
@@ -236,7 +237,8 @@ class GLMTarget(_Target):
     log pi(theta) = c0 + sum_i l_i(x_i' theta) - sum_d prior_prec[d] theta_d^2 / 2, with `family` "bernoulli_logit"
     (y in {0, 1}) or "poisson_log" (y in 0, 1, ...).  X is (n, D), an intercept is a column of ones; prior_prec is a
     scalar, a D-vector or None (flat prior).  Device-buffer phasepoint / step / static transitions with a Unit or Diag
-    metric and D <= 256 run the chain-tile kernel; everything else runs as a run-time compiled target (UserTarget)."""
+    metric and D <= 256 run the chain-tile kernel; everything else runs as a run-time compiled target (UserTarget),
+    the in-launch warm-ups included (Diag metric, or Dense with metric_estimator="welford_cov" or step size only)."""
 
     FAMILIES = {"bernoulli_logit": L.GLM_BERNOULLI_LOGIT, "poisson_log": L.GLM_POISSON_LOG}
 
@@ -1073,7 +1075,8 @@ class VectorisedStanAdaptor:
     or the static-HMC launch (ahmc_hmc_adapt_sample_f64).  metric_estimator: "welford" (`WelfordVar((D, N))` of the
     positions), "nutpie" (`NutpieVar((D, N))`, massmatrix.jl:172-250: positions and gradients) or, with a
     DenseEuclideanMetric (shared or per chain), "welford_cov" (one `WelfordCov(D)` per chain, massmatrix.jl:284-340).  A
-    Dense metric with adapt_metric = False adapts the step size only."""
+    Dense metric with adapt_metric = False adapts the step size only.  Every estimator runs on the built-in targets,
+    UserTarget and GLMTarget alike; CallbackTarget cannot adapt inside a launch."""
     delta: float = 0.8
     adapt_metric: bool = True
     init_buffer: int = 75

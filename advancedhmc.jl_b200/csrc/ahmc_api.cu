@@ -1408,17 +1408,14 @@ static int check_transition_io(ahmc_ctx* ctx, const ahmc_metric* metric, const a
 // sampler family checks of each entry point, the staging of the adaptors' buffers, and the per-chain workspace
 // The metric / estimator pairs an adaptive launch accepts, checked before everything else of the cfg: the diagonal
 // estimators adapt a Diag metric; a Dense metric (shared or per chain, as the starting point) adapts its step size only or
-// runs WelfordCov, on built-in targets.
-static int check_adapt_metric(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, const ahmc_adapt_cfg* cfg) {
+// runs WelfordCov, on built-in and run-time compiled targets alike (GLM targets adapt in their general form).
+static int check_adapt_metric(ahmc_ctx* ctx, const ahmc_adapt_cfg* cfg, const ahmc_metric* metric) {
     if (cfg->adapt_metric == AHMC_ADAPT_WELFORD_COV && metric->kind != AHMC_METRIC_DENSE)
         return fail(ctx, AHMC_ERR_INVALID, "cfg.adapt_metric = AHMC_ADAPT_WELFORD_COV adapts a dense M^-1: it needs the Dense metric");
     if (metric->kind == AHMC_METRIC_DENSE) {
         if (cfg->adapt_metric != AHMC_ADAPT_STEPSIZE && cfg->adapt_metric != AHMC_ADAPT_WELFORD_COV)
             return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation of a Dense metric: AHMC_ADAPT_STEPSIZE or AHMC_ADAPT_WELFORD_COV "
                                                    "(WelfordVar / NutpieVar estimate a diagonal M^-1)");
-        if (model->kind == AHMC_MODEL_USER)
-            return fail(ctx, AHMC_ERR_UNSUPPORTED, "in-launch adaptation with a Dense metric is built for the built-in targets; "
-                                                   "run-time compiled targets adapt a Diag metric");
         // the launch copies the starting factor into the chain's cholU_chain row (and reads the chain's row for every
         // momentum refresh), so it is required even with AHMC_FLAG_NO_REFRESH
         if (!metric->cholU)
@@ -1450,9 +1447,9 @@ static int check_adapt_cfg(ahmc_ctx* ctx, const ahmc_adapt_cfg* cfg, const ahmc_
 }
 // in-launch adaptation: the metric / estimator pair, then `refusal` (why this sampler configuration cannot adapt inside
 // its launch, or nullptr), then the cfg
-static int check_adapt(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* metric, const ahmc_adapt_cfg* cfg,
+static int check_adapt(ahmc_ctx* ctx, const ahmc_metric* metric, const ahmc_adapt_cfg* cfg,
                        const ahmc_rng* rng, int32_t n_transitions, const char* refusal) {
-    int rc = check_adapt_metric(ctx, model, metric, cfg);
+    int rc = check_adapt_metric(ctx, cfg, metric);
     if (rc) return rc;
     if (refusal) return fail(ctx, AHMC_ERR_UNSUPPORTED, "%s", refusal);
     return check_adapt_cfg(ctx, cfg, rng, n_transitions);
@@ -1515,7 +1512,7 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
     if (n_transitions < 1) return fail(ctx, AHMC_ERR_INVALID, "n_transitions must be >= 1");
     int rc;
     if (cfg &&
-        (rc = check_adapt(ctx, model, metric, cfg, rng, n_transitions,
+        (rc = check_adapt(ctx, metric, cfg, rng, n_transitions,
                           model->kind == AHMC_MODEL_CALLBACK
                               ? "in-launch adaptation needs a device-resident target: callback (split-step) models cannot run inside one launch; express the target as CUDA source (ahmc_model_create_user)"
                               : nullptr)))
@@ -1612,7 +1609,7 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
     if (!ctx || !model || !metric || !rng) return fail(ctx, AHMC_ERR_INVALID, "NULL ctx/model/metric/rng");
     if (n_transitions < 1) return fail(ctx, AHMC_ERR_INVALID, "n_transitions must be >= 1");
     int rc;
-    if (cfg && (rc = check_adapt(ctx, model, metric, cfg, rng, n_transitions,
+    if (cfg && (rc = check_adapt(ctx, metric, cfg, rng, n_transitions,
                                  (flags & (AHMC_FLAG_NUTS_SLICE_TS | AHMC_FLAG_NUTS_CLASSIC | AHMC_FLAG_NUTS_STRICT))
                                      ? "in-launch adaptation is built for MultinomialTS + GeneralisedNoUTurn"
                                      : nullptr)))

@@ -341,7 +341,7 @@ cudaError_t launch_hmc_big(const HmcArgs& a, cudaStream_t st) {
     };
     if (!a.ad.enabled) return run(IC<0>{}, BigMetrics{});
     // the adaptive form: Diag metric only (the chain adapts its diagonal M^-1)
-    if (adapt_form(a.ad) == AHMC_ADAPT_NUTPIE) return run(IC<AHMC_ADAPT_NUTPIE>{}, Kinds<AHMC_METRIC_DIAG>{});
+    if (adapt_kernel(a.ad, a.lf.metric).form == AHMC_ADAPT_NUTPIE) return run(IC<AHMC_ADAPT_NUTPIE>{}, Kinds<AHMC_METRIC_DIAG>{});
     return run(IC<AHMC_ADAPT_WELFORD>{}, Kinds<AHMC_METRIC_DIAG>{});
 }
 

@@ -135,12 +135,18 @@ inline bool stan_window_schedule(AdaptDev& ad, int init_buffer, int term_buffer,
     return true;
 }
 
-// the compiled estimator form (ahmc_chain_adapt.cuh) an adaptive launch needs: NutpieVar has its own, step size only and
-// WelfordVar share one
-inline int adapt_form(const AdaptDev& ad) { return ad.adapt_metric == AHMC_ADAPT_NUTPIE ? AHMC_ADAPT_NUTPIE : AHMC_ADAPT_WELFORD; }
-// the form for a Dense metric (step size only or WelfordCov)
-inline int adapt_form(const AdaptDev& ad, int metric_kind) {
-    return metric_kind == AHMC_METRIC_DENSE ? AHMC_ADAPT_WELFORD_COV : adapt_form(ad);
+// The kernel instantiation an adaptive launch runs: the template metric kind and the compiled estimator form
+// (ahmc_chain_adapt.cuh).  A Diag metric runs on the Diag kind with NutpieVar's form or the one that step size only and
+// WelfordVar share; a Dense metric, shared or per chain (the starting point), runs on the chain's own rows
+// (kMetricDenseChain) with the WelfordCov form, step size only included.  The one decision for the built-in targets and
+// the run-time compiled ones (launch_hmc, launch_nuts).
+struct AdaptKernel {
+    int metric_kind;
+    int form;
+};
+inline AdaptKernel adapt_kernel(const AdaptDev& ad, const MetricDev& metric) {
+    if (metric.kind == AHMC_METRIC_DENSE) return {kMetricDenseChain, AHMC_ADAPT_WELFORD_COV};
+    return {metric.kind, ad.adapt_metric == AHMC_ADAPT_NUTPIE ? AHMC_ADAPT_NUTPIE : AHMC_ADAPT_WELFORD};
 }
 
 struct HmcArgs {
@@ -350,7 +356,8 @@ struct UserModule;  // per-model cache of compiled kernels
 UserModule* user_module_create(const char* cuda_src, char* err, size_t err_len);
 void user_module_destroy(UserModule* m);
 // compile (first use) and launch kernel `which` of the user module for (metric, G, E); args = the kernel's argument block
-// form: the estimator form of an adaptive kernel (UK_NUTS_ADAPT / UK_HMC_ADAPT: adapt_form(ad)), 0 for the others
+// metric_kind: the template kind (metric_form; adaptive kernels: adapt_kernel's); form: the estimator form of an adaptive
+// kernel (UK_NUTS_ADAPT / UK_HMC_ADAPT: adapt_kernel's), 0 for the others
 cudaError_t user_launch(UserModule* m, int which, int metric_kind, int G, int E, const void* args, unsigned blocks, size_t smem,
                         cudaStream_t st, int form = 0);
 const char* user_last_error(const UserModule* m);

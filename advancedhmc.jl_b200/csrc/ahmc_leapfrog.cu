@@ -668,9 +668,10 @@ static cudaError_t launch_lf_t(const LeapfrogArgs& a, cudaStream_t st) {
 }
 
 // the entry points with a D > 512 streaming form and a run-time compiled form: past D = 512 `big`, for a user target its
-// compiled kernel `uk` (estimator form `form`), else `builtin(G, E)` at the register-resident layout of D
+// compiled kernel `uk` on the template metric kind `metric_kind` (estimator form `form`), else `builtin(G, E)` at the
+// register-resident layout of D
 template <class Args, class Builtin>
-static cudaError_t front_door(const Args& a, int D, long long N, const ModelDev& model, const MetricDev& metric,
+static cudaError_t front_door(const Args& a, int D, long long N, const ModelDev& model, int metric_kind,
                               cudaError_t (*big)(const Args&, cudaStream_t), int uk, int form, cudaStream_t st,
                               int* n_launches, Builtin&& builtin) {
     int G, E;
@@ -682,21 +683,21 @@ static cudaError_t front_door(const Args& a, int D, long long N, const ModelDev&
     if (n_launches) *n_launches += 1;
     if (model.kind == AHMC_MODEL_USER) {  // run-time compiled kernels of a user target (ahmc_user.cu)
         const int cpb = kBlockThreads / G;
-        return user_launch((UserModule*)model.user, uk, metric_form(metric), G, E, &a, (unsigned)((N + cpb - 1) / cpb),
-                           smem_bytes(AHMC_MODEL_USER, metric.kind, D, G), st, form);
+        return user_launch((UserModule*)model.user, uk, metric_kind, G, E, &a, (unsigned)((N + cpb - 1) / cpb),
+                           smem_bytes(AHMC_MODEL_USER, metric_kind, D, G), st, form);
     }
     return builtin(G, E);
 }
 
 cudaError_t launch_leapfrog(const LeapfrogArgs& a, cudaStream_t st, int* n_launches) {
-    return front_door(a, a.D, a.N, a.model, a.metric, launch_leapfrog_big, UK_LEAPFROG, 0, st, n_launches, [&](int G, int E) {
+    return front_door(a, a.D, a.N, a.model, metric_form(a.metric), launch_leapfrog_big, UK_LEAPFROG, 0, st, n_launches, [&](int G, int E) {
         return with_model_metric_layout(AllModels{}, AllMetrics{}, a.model.kind, metric_form(a.metric), G, E,
                                         [&](auto M, auto K, auto g, auto e) { return launch_lf_t<M, K, g, e>(a, st); });
     });
 }
 
 cudaError_t launch_find_eps(const FindEpsArgs& a, cudaStream_t st, int* n_launches) {
-    return front_door(a, a.D, a.N, a.model, a.metric, launch_find_eps_big, UK_FIND_EPS, 0, st, n_launches, [&](int G, int E) {
+    return front_door(a, a.D, a.N, a.model, metric_form(a.metric), launch_find_eps_big, UK_FIND_EPS, 0, st, n_launches, [&](int G, int E) {
         return with_model_metric_layout(AllModels{}, AllMetrics{}, a.model.kind, metric_form(a.metric), G, E, [&](auto M, auto K, auto g, auto e) {
             return launch_warps(find_eps_kernel<M, K, g, e>, a.N, g, smem_bytes(M, K, a.D, g), st, a);
         });
@@ -704,7 +705,7 @@ cudaError_t launch_find_eps(const FindEpsArgs& a, cudaStream_t st, int* n_launch
 }
 
 cudaError_t launch_phasepoint(const PhasepointArgs& a, cudaStream_t st, int* n_launches) {
-    return front_door(a, a.D, a.N, a.model, a.metric, launch_phasepoint_big, UK_PHASEPOINT, 0, st, n_launches, [&](int G, int E) {
+    return front_door(a, a.D, a.N, a.model, metric_form(a.metric), launch_phasepoint_big, UK_PHASEPOINT, 0, st, n_launches, [&](int G, int E) {
         return with_model_metric_layout(AllModels{}, AllMetrics{}, a.model.kind, metric_form(a.metric), G, E, [&](auto M, auto K, auto g, auto e) {
             return launch_warps(phasepoint_kernel<M, K, g, e>, a.N, g, smem_bytes(M, K, a.D, g), st, a);
         });
@@ -713,18 +714,21 @@ cudaError_t launch_phasepoint(const PhasepointArgs& a, cudaStream_t st, int* n_l
 
 cudaError_t launch_hmc(const HmcArgs& a, cudaStream_t st, int* n_launches) {
     const LeapfrogArgs& lf = a.lf;
-    return front_door(a, lf.D, lf.N, lf.model, lf.metric, launch_hmc_big, a.ad.enabled ? UK_HMC_ADAPT : UK_HMC,
-                      a.ad.enabled ? adapt_form(a.ad) : 0, st, n_launches, [&](int G, int E) -> cudaError_t {
-        auto run = [&](auto form, auto metrics, int metric) {
-            return with_model_metric_layout(AllModels{}, metrics, lf.model.kind, metric, G, E, [&](auto M, auto K, auto g, auto e) {
+    const AdaptKernel ak = a.ad.enabled ? adapt_kernel(a.ad, lf.metric) : AdaptKernel{metric_form(lf.metric), 0};
+    return front_door(a, lf.D, lf.N, lf.model, ak.metric_kind, launch_hmc_big, a.ad.enabled ? UK_HMC_ADAPT : UK_HMC, ak.form, st,
+                      n_launches, [&](int G, int E) -> cudaError_t {
+        auto run = [&](auto form, auto metrics) {
+            return with_model_metric_layout(AllModels{}, metrics, lf.model.kind, ak.metric_kind, G, E, [&](auto M, auto K, auto g, auto e) {
                 return launch_warps(hmc_kernel<M, K, g, e, form>, lf.N, g, smem_bytes(M, K, lf.D, g), st, a);
             });
         };
-        if (!a.ad.enabled) return run(IC<0>{}, AllMetrics{}, metric_form(lf.metric));
         // the adaptive forms run on the metric their estimator adapts: Diag, or for WelfordCov the chain's own Dense rows
-        if (lf.metric.kind == AHMC_METRIC_DENSE) return run(IC<AHMC_ADAPT_WELFORD_COV>{}, Kinds<kMetricDenseChain>{}, kMetricDenseChain);
-        if (adapt_form(a.ad) == AHMC_ADAPT_NUTPIE) return run(IC<AHMC_ADAPT_NUTPIE>{}, Kinds<AHMC_METRIC_DIAG>{}, lf.metric.kind);
-        return run(IC<AHMC_ADAPT_WELFORD>{}, Kinds<AHMC_METRIC_DIAG>{}, lf.metric.kind);
+        switch (ak.form) {
+            case 0: return run(IC<0>{}, AllMetrics{});
+            case AHMC_ADAPT_WELFORD_COV: return run(IC<AHMC_ADAPT_WELFORD_COV>{}, Kinds<kMetricDenseChain>{});
+            case AHMC_ADAPT_NUTPIE: return run(IC<AHMC_ADAPT_NUTPIE>{}, Kinds<AHMC_METRIC_DIAG>{});
+            default: return run(IC<AHMC_ADAPT_WELFORD>{}, Kinds<AHMC_METRIC_DIAG>{});
+        }
     });
 }
 

@@ -29,18 +29,25 @@ cudaError_t launch_nuts_cov(const NutsArgs& a, cudaStream_t st);       // ahmc_n
 
 cudaError_t launch_nuts(const NutsArgs& a, cudaStream_t st, int* n_launches) {
     if (n_launches) *n_launches += 1;
+    // (adaptive: the metric kind and estimator form of the instantiation, decided once for both kinds of target)
+    const AdaptKernel ak = a.ad.enabled ? adapt_kernel(a.ad, a.metric) : AdaptKernel{metric_form(a.metric), 0};
     if (a.model.kind == AHMC_MODEL_USER) {  // run-time compiled kernel of a user target (default / adaptive family, ahmc_user.cu)
         int G, E;
         if (!pick_layout(a.D, &G, &E) || a.sampler != 0 || a.criterion != 0) return cudaErrorInvalidValue;
-        if (a.ad.enabled && a.metric.kind != AHMC_METRIC_DIAG) return cudaErrorInvalidValue;
+        if (a.ad.enabled && a.metric.kind != AHMC_METRIC_DIAG && a.metric.kind != AHMC_METRIC_DENSE) return cudaErrorInvalidValue;
         const int cpb = kBlockThreads / G;
         const int maxd = a.max_depth > 0 ? a.max_depth : 1;
-        const size_t sm = smem_bytes(AHMC_MODEL_USER, a.metric.kind, a.D, G) + (size_t)cpb * maxd * kLevelScalars * sizeof(double);
-        return user_launch((UserModule*)a.model.user, a.ad.enabled ? UK_NUTS_ADAPT : UK_NUTS, metric_form(a.metric), G, E, &a,
-                           (unsigned)((a.N + cpb - 1) / cpb), sm, st, a.ad.enabled ? adapt_form(a.ad) : 0);
+        const size_t sm = smem_bytes(AHMC_MODEL_USER, ak.metric_kind, a.D, G) + (size_t)cpb * maxd * kLevelScalars * sizeof(double);
+        return user_launch((UserModule*)a.model.user, a.ad.enabled ? UK_NUTS_ADAPT : UK_NUTS, ak.metric_kind, G, E, &a,
+                           (unsigned)((a.N + cpb - 1) / cpb), sm, st, ak.form);
     }
-    if (a.ad.enabled && a.metric.kind == AHMC_METRIC_DENSE) return launch_nuts_cov(a, st);
-    if (a.ad.enabled) return a.ad.adapt_metric == AHMC_ADAPT_NUTPIE ? launch_nuts_nutpie(a, st) : launch_nuts_adaptive(a, st);
+    if (a.ad.enabled) {
+        switch (ak.form) {
+            case AHMC_ADAPT_WELFORD_COV: return launch_nuts_cov(a, st);
+            case AHMC_ADAPT_NUTPIE: return launch_nuts_nutpie(a, st);
+            default: return launch_nuts_adaptive(a, st);
+        }
+    }
     if (a.sampler != 0 || a.criterion != 0) return launch_nuts_variants(a, st);
     return nuts_dispatch<false, false, false>(a, st);
 }

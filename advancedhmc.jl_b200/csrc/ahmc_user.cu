@@ -257,14 +257,25 @@ int user_source_check(const char* cuda_src, int which, int metric_kind, int D, c
     if (!pick_layout(D, &G, &E)) return -1;
     UserModule m;
     m.src = cuda_src;
-    // the adaptive kernels: both estimator forms
+    // the adaptive kernels: every instantiation a launch with this metric can pick (adapt_kernel) -- for a Diag metric both
+    // estimator forms, for a Dense one the WelfordCov form on the chain's own rows
     const bool adaptive = which == UK_NUTS_ADAPT || which == UK_HMC_ADAPT;
-    for (int form : {adaptive ? AHMC_ADAPT_WELFORD : 0, adaptive ? AHMC_ADAPT_NUTPIE : 0}) {
-        if (!compile(&m, which, metric_kind, G, E, form, nullptr)) {
+    std::vector<AdaptKernel> kernels{{metric_kind, 0}};
+    if (adaptive) {
+        AdaptDev ad{};
+        const MetricDev md{metric_kind};
+        kernels.clear();
+        for (int est : {AHMC_ADAPT_WELFORD, AHMC_ADAPT_NUTPIE}) {
+            ad.adapt_metric = est;
+            const AdaptKernel k = adapt_kernel(ad, md);
+            if (kernels.empty() || kernels.back().form != k.form) kernels.push_back(k);
+        }
+    }
+    for (const AdaptKernel& k : kernels) {
+        if (!compile(&m, which, k.metric_kind, G, E, k.form, nullptr)) {
             if (log) snprintf(log, log_len, "%s", m.err.c_str());
             return -1;
         }
-        if (!adaptive) break;
     }
     return 0;
 }

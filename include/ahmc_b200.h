@@ -299,9 +299,10 @@ int ahmc_nuts_sample_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metr
  * D x N variance, i.e. a per-chain diagonal M^-1), scheduled like `StanHMCAdaptor` (stan_adaptor.jl:13-50, 137-159: windows, reset of both
  * adaptors at each window end, `finalize!` eps = exp(x_bar) after iteration n_adapts).  Because nothing is pooled,
  * chains never wait for each other: iterations 1..n_adapts adapt, n_adapts+1..n_transitions sample with the final
- * eps / M^-1.  Requires the Diag metric (shared or per-chain M^-1 as the starting point) or, on built-in targets, the
- * Dense metric (shared or per chain) with AHMC_ADAPT_STEPSIZE or AHMC_ADAPT_WELFORD_COV; MultinomialTS +
- * GeneralisedNoUTurn, Philox randomness (no tapes).  Dense with WelfordVar / NutpieVar, and Dense on run-time compiled
+ * eps / M^-1.  Requires the Diag metric (shared or per-chain M^-1 as the starting point) or the Dense metric (shared or
+ * per chain) with AHMC_ADAPT_STEPSIZE or AHMC_ADAPT_WELFORD_COV, on built-in and run-time compiled targets alike (a GLM
+ * target adapts in its general, run-time compiled form); MultinomialTS + GeneralisedNoUTurn, Philox randomness (no
+ * tapes), D <= 512 for a Dense metric or a run-time compiled target.  Dense with WelfordVar / NutpieVar, and callback
  * targets: AHMC_ERR_UNSUPPORTED; AHMC_ADAPT_WELFORD_COV with a Unit or Diag metric: AHMC_ERR_INVALID.
  * With AHMC_ADAPT_WELFORD_COV chain c behaves like `sample(h_c, NUTS, n; adaptor = StanHMCAdaptor(WelfordCov(D),
  * NesterovDualAveraging(delta, eps_c)))`: the launch copies the starting metric into the chain's Minv_chain / cholU_chain

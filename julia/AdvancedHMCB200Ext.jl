@@ -68,7 +68,7 @@ struct CAdaptCfg
     delta::Float64; gamma::Float64; t0::Float64; kappa::Float64
     adapt_metric::Int32; n_min::Int32
     eps_chain::Ptr{Float64}; Minv_chain::Ptr{Float64}; eps_trace::Ptr{Float64}
-    cholU_chain::Ptr{Float64}  # AHMC_ADAPT_WELFORD_COV (adapt_metric = 3): N x D x D upper factors, out
+    cholU_chain::Ptr{Float64}  # AHMC_ADAPT_WELFORD_COV (adapt_metric = 3, Dense metric, any device-resident target): N x D x D upper factors, out
 end
 struct CPooledCfg
     n_adapts::Int32; init_buffer::Int32; term_buffer::Int32; window_size::Int32
@@ -187,7 +187,9 @@ end
 Generalised linear model with a Gaussian prior (ahmc_model_create_glm): `family` 0 = Bernoulli-logit, 1 = Poisson-log,
 `X` n × D (row `i` is `x_i`; copied row-major), `prior_prec` a D-vector or `nothing` (flat prior).  On the reference side
 this is `Hamiltonian(metric, ℓπ, ∂ℓπ∂θ)` with ℓπ(θ) = c0 + Σᵢ lᵢ(xᵢ'θ) − Σ_d prior_prec[d] θ_d²/2 and its gradient.
-Like the rest of this shim it has not been executed (no Julia on the build machines).
+In-launch warm-up runs it in its general form, with a Diag metric or with a Dense one (step size only or one `WelfordCov`
+per chain), as for the built-in targets.  Like the rest of this shim it has not been executed (no Julia on the build
+machines).
 """
 function B200GLMTarget(X::Matrix{Float64}, y::Vector{Float64}; family::Integer=0, prior_prec=nothing, c0=0.0)
     n, D = size(X)
