@@ -27,8 +27,8 @@ constexpr int kKC = 16;             // columns of A per pipeline stage
 //     16-column chunk is ONE contiguous bulk copy instead of sixteen;
 //   * consumers release a stage through an "empty" mbarrier (one arrival per warp) and only the producer thread waits on it,
 //     instead of a CTA-wide __syncthreads per chunk;
-//   * three stages.  Shared memory: 68 KB per CTA at Dp = 128 (two CTAs per SM still fit), 232,272 of the 232,448 bytes a CTA
-//     may have at Dp = 512.
+//   * three stages.  Shared memory (dense_smem_bytes): 68 KB per CTA at Dp = 128 (two CTAs per SM still fit), 232,240
+//     dynamic + 8 static of the 232,448 bytes a CTA may have at Dp = 512.
 constexpr int kStages = 3;  // the wait is L2 latency per chunk, not pipeline depth
 constexpr int kBars = 2 * kStages;  // full[kStages] + empty[kStages]
 #ifdef AHMC_SIMT_EMULATION
@@ -394,6 +394,13 @@ __global__ void vec_norm_kernel(const double* __restrict__ v, int D, double* nor
     }
 }
 
+// dynamic shared memory of a K4 launch, exactly its layout: kStages stages of kKC columns, the tile's vectors (CT x Dx), the
+// per-warp energy partials ([8 warps][CT][2]) and the kBars mbarriers
+__host__ inline size_t dense_smem_bytes(int Dp, int CB) {
+    const size_t CT = 8 * (size_t)CB, Ds = (size_t)Dp + 4;
+    return ((size_t)kStages * kKC * Ds + CT * Ds + 8 * CT * 2) * sizeof(double) + kBars * sizeof(uint64_t);
+}
+
 bool dense_tile_shape(int D, int* Dp, int* RB, int* CB) {
     if (D < 1 || D > 512) return false;
     *Dp = ((D + 63) / 64) * 64;
@@ -415,9 +422,7 @@ cudaError_t launch_vec_norm(const double* v, int D, double* norm, cudaStream_t s
 template <int RB, int CB, int MINB = 1>
 static cudaError_t launch_dense_t(const DenseArgs& a, cudaStream_t st) {
     constexpr int CT = 8 * CB;
-    const int Ds = a.Dp + 4;
-    const size_t sm = ((size_t)kStages * kKC * Ds + (size_t)CT * Ds + 8 * CT * 2) * sizeof(double) + 64;
-    return launch_kernel(dense_traj_kernel<RB, CB, MINB>, (a.N + CT - 1) / CT, kDenseThreads, sm, st, a);
+    return launch_kernel(dense_traj_kernel<RB, CB, MINB>, (a.N + CT - 1) / CT, kDenseThreads, dense_smem_bytes(a.Dp, CB), st, a);
 }
 
 cudaError_t launch_dense_traj(const DenseTrajHost& h, cudaStream_t st, int* n_launches) {

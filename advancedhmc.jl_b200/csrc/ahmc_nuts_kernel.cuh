@@ -747,22 +747,33 @@ __global__ void __launch_bounds__(COOP ? kCoopThreads : kBlockThreads, COOP ? 1 
 
 }
 
+#ifndef __CUDACC_RTC__
+// dynamic shared memory of a NUTS launch: with `coop` (dense operators, one chain per warp, default family) the
+// cooperative products' pipeline (coop_smem_doubles), otherwise the groups' operator slabs (smem_bytes); then every
+// group's level scalars
+template <int E>
+__host__ inline size_t nuts_smem_bytes(bool coop, int model_kind, int metric_kind, int D, int G, int max_depth) {
+    const int maxd = max_depth > 0 ? max_depth : 1;
+    if (coop) return ((size_t)coop_smem_doubles(D, coop_kc<E>()) + (size_t)kCoopWarps * maxd * kLevelScalars) * sizeof(double);
+    return smem_bytes(model_kind, metric_kind, D, G) + (size_t)(kBlockThreads / G) * maxd * kLevelScalars * sizeof(double);
+}
+#endif
+
 #if !defined(AHMC_SIMT_EMULATION) && !defined(__CUDACC_RTC__)  // host launch code (skipped by the CPU SIMT emulation harness and by NVRTC)
 template <int MODEL, int METRIC, int G, int E, bool VAR, int ADAPT>
 static cudaError_t launch_nuts_v(const NutsArgs& a, cudaStream_t st) {
-    const int maxd = a.max_depth > 0 ? a.max_depth : 1;
     // (a per-chain Dense metric, kMetricDenseChain, has no shared matrix: it always runs warp per chain)
     constexpr bool kDenseOps = (MODEL == AHMC_MODEL_DENSE_GAUSS || METRIC == AHMC_METRIC_DENSE) && METRIC != kMetricDenseChain;
     if constexpr (kDenseOps && G == 32 && !VAR) {
         // dense operators, one chain per warp: blocks of kCoopWarps chains share every D x D product (COOP form)
         const long long blocks = (a.N + kCoopWarps - 1) / kCoopWarps;
-        const size_t sm = ((size_t)coop_smem_doubles(a.D, coop_kc<E>()) + (size_t)kCoopWarps * maxd * kLevelScalars) * sizeof(double);
+        const size_t sm = nuts_smem_bytes<E>(true, MODEL, METRIC, a.D, G, a.max_depth);
         if constexpr (E >= 2 && E <= 8) {
             if (a.D == G * E) return launch_kernel(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, true, true>, blocks, kCoopThreads, sm, st, a);
         }
         return launch_kernel(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, false, true>, blocks, kCoopThreads, sm, st, a);
     } else {
-        const size_t sm = smem_bytes(MODEL, METRIC, a.D, G) + (size_t)(kBlockThreads / G) * maxd * kLevelScalars * sizeof(double);
+        const size_t sm = nuts_smem_bytes<E>(false, MODEL, METRIC, a.D, G, a.max_depth);
         if constexpr (G == 32 && E >= 2 && E <= 8) {
             if (a.D == G * E) return launch_warps(nuts_kernel<MODEL, METRIC, G, E, VAR, ADAPT, true>, a.N, G, sm, st, a);  // full tile: compile-time D
         }

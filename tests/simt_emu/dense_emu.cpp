@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "ahmc_dense.cu"
+#include "emu_smem.h"
 
 void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 
@@ -16,6 +17,7 @@ namespace ahmc {
 unsigned char* emu_dynamic_smem = nullptr;
 // (the mbarrier / bulk-copy / DMMA contracts live in simt_emu.cpp: the cooperative NUTS products use them too)
 }  // namespace ahmc
+EMU_DEFINE_SMEM_ARENA();
 using namespace ahmc;
 
 template <int RB, int CB, int MINB>
@@ -56,8 +58,8 @@ struct EmuDense {
 extern "C" int emu_dense_stages() { return kStages; }
 extern "C" int emu_dense(EmuDense* q) {
     // (mbarrier table: reset per block by emu_launch)
-    int Dp, RB, CB;
-    if (!dense_tile_shape(q->D, &Dp, &RB, &CB)) return -1;
+    int Dp, RB, CB_shape;
+    if (!dense_tile_shape(q->D, &Dp, &RB, &CB_shape)) return -1;
     std::vector<double> Pp, Mp;
     double norms[2] = {0.0, 0.0};
     PadArgs pa{};
@@ -86,17 +88,22 @@ extern "C" int emu_dense(EmuDense* q) {
     a.th_out = q->th_out; a.r_out = q->r_out; a.g_out = q->g_out; a.dr_out = q->dr_out; a.lp_out = q->lp_out; a.lk_out = q->lk_out;
     a.ld_out = q->D; a.status = q->status; a.steps_done = q->steps_done; a.need_exact = q->need_exact;
     void (*fn)(const void*) = nullptr;
-    int CT = 0;
-    if (RB == 1) fn = dense_thunk<1, 4, 1>, CT = 32;
-    else if (RB == 2 && q->wide_tile) fn = dense_thunk<2, 4, 1>, CT = 32;
-    else if (RB == 2) fn = dense_thunk<2, 2, 2>, CT = 16;
-    else if (RB == 3) fn = dense_thunk<3, 2, 1>, CT = 16;
+    int CB = 0;  // the instantiation's, as launch_dense_traj picks it (RB == 2 may ask for the 32-chain form instead)
+    if (RB == 1) fn = dense_thunk<1, 4, 1>, CB = 4;
+    else if (RB == 2 && q->wide_tile) fn = dense_thunk<2, 4, 1>, CB = 4;
+    else if (RB == 2) fn = dense_thunk<2, 2, 2>, CB = 2;
+    else if (RB == 3) fn = dense_thunk<3, 2, 1>, CB = 2;
+    else if (RB == 4) fn = dense_thunk<4, 2, 1>, CB = 2;
+    else if (RB == 5) fn = dense_thunk<5, 1, 1>, CB = 1;
+    else if (RB == 6) fn = dense_thunk<6, 1, 1>, CB = 1;
+    else if (RB == 7) fn = dense_thunk<7, 1, 1>, CB = 1;
+    else if (RB == 8) fn = dense_thunk<8, 1, 1>, CB = 1;
     else return -2;
-    const int Ds = Dp + 4;
-    const size_t sm = ((size_t)kStages * kKC * Ds + (size_t)CT * Ds + 8 * CT * 2) * sizeof(double) + 64;  // as launch_dense_t
-    std::vector<double> smem(sm / sizeof(double) + 2, 0.0);
-    emu_dynamic_smem = reinterpret_cast<unsigned char*>(smem.data());
+    const int CT = 8 * CB;
+    emu_dynamic_smem = emu_smem_base();
+    emu_smem_begin(emu_dynamic_smem, dense_smem_bytes(Dp, CB), 2 * sizeof(int) /* s_flag, s_k */, "dense_traj_kernel");
     emu_launch(fn, &a, (int)((q->N + CT - 1) / CT), kDenseThreads);
+    emu_smem_end();
     emu_dynamic_smem = nullptr;
     return 0;
 }

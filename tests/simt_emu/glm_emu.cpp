@@ -7,12 +7,14 @@
 #include <vector>
 
 #include "ahmc_glm.cu"
+#include "emu_smem.h"
 
 void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 
 namespace ahmc {
 unsigned char* emu_dynamic_smem = nullptr;
 }
+EMU_DEFINE_SMEM_ARENA();
 using namespace ahmc;
 
 template <int RB, int CB, int FAM>
@@ -57,9 +59,10 @@ extern "C" int emu_glm(EmuGlm* e) {
     else if (RB == 2) fn = logit ? glm_thunk<2, 2, 0> : glm_thunk<2, 2, 1>;
     else if (RB == 3) fn = logit ? glm_thunk<3, 2, 0> : glm_thunk<3, 2, 1>;
     else fn = logit ? glm_thunk<4, 2, 0> : glm_thunk<4, 2, 1>;
-    std::vector<double> smem(sm / sizeof(double) + 2, 0.0);
-    emu_dynamic_smem = reinterpret_cast<unsigned char*>(smem.data());
+    emu_dynamic_smem = emu_smem_base();
+    emu_smem_begin(emu_dynamic_smem, sm, 0, "glm_traj_kernel");
     emu_launch(fn, &a, (int)((e->N + 8 * CB - 1) / (8 * CB)), kGlmThreads);
+    emu_smem_end();
     emu_dynamic_smem = nullptr;
     return 0;
 }

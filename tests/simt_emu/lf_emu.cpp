@@ -5,10 +5,9 @@
 #include <vector>
 
 #include "ahmc_leapfrog.cu"
+#include "emu_smem.h"
 
-namespace ahmc {
-double smem[1 << 16];
-}
+EMU_DEFINE_SMEM_ARENA();  // the block's dynamic shared memory (`extern __shared__ double smem[]` in the kernels)
 void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 using namespace ahmc;
 
@@ -101,6 +100,10 @@ extern "C" int emu_leapfrog(const EmuLf* q) {
     if (!fn) return -2;
     const int chains_per_block = kBlockThreads / G;
     const int blocks = (int)((q->N + chains_per_block - 1) / chains_per_block);
+    // K1's exact path and K2 use one operator slab per group (the pair kernel: per warp, as G = 32 does); the launcher's
+    // occupancy padding for host-memory lanes only adds bytes the kernel never touches
+    emu_smem_begin(emu_smem_base(), smem_bytes(m, me, D, G), 0, hm ? "hmc_kernel" : "leapfrog_kernel");
     emu_launch(fn, hm ? (const void*)&h : (const void*)&a, blocks, kBlockThreads);
+    emu_smem_end();
     return 0;
 }

@@ -6,10 +6,9 @@
 #include <vector>
 
 #include "ahmc_nuts_kernel.cuh"
+#include "emu_smem.h"
 
-namespace ahmc {
-double smem[1 << 16];  // the block's dynamic shared memory (`extern __shared__ double smem[]` in the kernel)
-}
+EMU_DEFINE_SMEM_ARENA();  // the block's dynamic shared memory (`extern __shared__ double smem[]` in the kernel)
 void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 
 using namespace ahmc;
@@ -76,9 +75,10 @@ static KernelFn by_layout(int G, int E) {
     if (G == 8 && E == 1) return thunk<MODEL, METRIC, 8, 1, VAR, ADAPT>;
     if (G == 32 && E == 2) return thunk<MODEL, METRIC, 32, 2, VAR, ADAPT>;
     if (G == 16 && E == 1) return thunk<MODEL, METRIC, 16, 1, VAR, ADAPT>;
+    if (G == 32 && E == 1) return thunk<MODEL, METRIC, 32, 1, VAR, ADAPT>;  // D in (16, 32]
     if (G == 32 && E == 4) return thunk<MODEL, METRIC, 32, 4, VAR, ADAPT>;
     if (G == 32 && E == 8) return thunk<MODEL, METRIC, 32, 8, VAR, ADAPT>;
-    if constexpr (MODEL == AHMC_MODEL_DENSE_GAUSS && METRIC == AHMC_METRIC_DENSE && !VAR && !ADAPT) {
+    if constexpr (!VAR && !ADAPT) {
         if (G == 32 && E == 16) return thunk<MODEL, METRIC, 32, 16, VAR, ADAPT>;  // D in (256, 512]: 16-column chunks, 2 stages
     }
     return nullptr;
@@ -97,6 +97,8 @@ static KernelFn by_model(int model, int metric, int G, int E) {
         if (!VAR) {  // the other two dense-operator combinations of the COOP form
             if (model == AHMC_MODEL_DENSE_GAUSS && metric == AHMC_METRIC_DIAG) return by_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DIAG, false, false>(G, E);
             if (model == AHMC_MODEL_DIAG_GAUSS && metric == AHMC_METRIC_DENSE) return by_layout<AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DENSE, false, false>(G, E);
+            if (model == AHMC_MODEL_DENSE_GAUSS && metric == AHMC_METRIC_UNIT) return by_layout<AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT, false, false>(G, E);
+            if (model == AHMC_MODEL_FUNNEL && metric == AHMC_METRIC_DENSE) return by_layout<AHMC_MODEL_FUNNEL, AHMC_METRIC_DENSE, false, false>(G, E);
         }
     }
     return nullptr;
@@ -118,7 +120,8 @@ extern "C" int emu_nuts(const EmuNuts* q) {
     if (D <= 4) G = 4, E = 1;
     else if (D <= 8) G = 8, E = 1;
     else if (D <= 16) G = 16, E = 1;
-    else if (D > 32 && D <= 64) G = 32, E = 2;
+    else if (D <= 32) G = 32, E = 1;  // (pick_layout, ahmc_leapfrog.cu)
+    else if (D <= 64) G = 32, E = 2;
     else if (D > 64 && D <= 128) G = 32, E = 4;  // the headline layout
     else if (D > 128 && D <= 256) G = 32, E = 8;  // C5's layout
     else if (D > 256 && D <= 512) G = 32, E = 16;
@@ -191,6 +194,16 @@ extern "C" int emu_nuts(const EmuNuts* q) {
     const int threads = coop ? kCoopThreads : kBlockThreads;
     const int chains_per_block = threads / G;
     const int blocks = (int)((q->N + chains_per_block - 1) / chains_per_block);
+    size_t sm = 0;  // what launch_nuts_v asks for
+    switch (E) {
+        case 1: sm = nuts_smem_bytes<1>(coop, q->model_kind, q->metric_kind, D, G, q->max_depth); break;
+        case 2: sm = nuts_smem_bytes<2>(coop, q->model_kind, q->metric_kind, D, G, q->max_depth); break;
+        case 4: sm = nuts_smem_bytes<4>(coop, q->model_kind, q->metric_kind, D, G, q->max_depth); break;
+        case 8: sm = nuts_smem_bytes<8>(coop, q->model_kind, q->metric_kind, D, G, q->max_depth); break;
+        default: sm = nuts_smem_bytes<16>(coop, q->model_kind, q->metric_kind, D, G, q->max_depth); break;
+    }
+    emu_smem_begin(emu_smem_base(), sm, 0, coop ? "nuts_kernel (COOP)" : "nuts_kernel");
     emu_launch(fn, &a, blocks, threads);
+    emu_smem_end();
     return 0;
 }

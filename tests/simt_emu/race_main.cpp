@@ -3,7 +3,8 @@
 // asks for (shuffles / votes / __syncwarp -> the warp's barrier, __syncthreads -> the block's, mbarriers and atomics ->
 // std::atomic_ref), so a missing barrier or fence in the kernel is a data race TSan reports -- the CPU counterpart of
 // compute-sanitizer's racecheck, and it also covers the staged compile-time variants that have not run on a GPU yet.
-// Build: -DRACE_NUTS, -DRACE_DENSE, -DRACE_LF, -DRACE_MN or -DRACE_ADAPT (plus the variant's -D knobs).  TEST INFRASTRUCTURE ONLY (tests/test_simt_emulation.py).
+// Build: -DRACE_NUTS, -DRACE_DENSE, -DRACE_LF, -DRACE_MN, -DRACE_ADAPT or -DRACE_GLM (plus the variant's -D knobs); the same
+// mains also run under AddressSanitizer (tests/test_tensor_pipe_shapes_cpu.py).  TEST INFRASTRUCTURE ONLY (tests/test_simt_emulation.py).
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -268,6 +269,33 @@ int main() {
     std::printf("adapt D %d N %lld: rc %d n %.0f\n", D, N, rc, rec[0]);
     return rc != 0 || rec[0] != (double)N;
 }
+#elif defined(RACE_GLM)
+#include "glm_emu.cpp"
+
+// K6: a 9-coordinate Bernoulli-logit target with 70 rows (two chunks, a partial last one), a ragged second tile
+int main() {
+    const int D = 9, n = 70, N = 17, steps = 2;
+    std::vector<double> X((size_t)n * D), y(n), prec(D, 1.0), th((size_t)N * D), r((size_t)N * D), o((size_t)6 * N * D), lp(N), lk(N);
+    std::vector<uint32_t> status(N);
+    std::vector<int32_t> done(N);
+    srand(3);
+    auto u = [] { return rand() / (double)RAND_MAX - 0.5; };
+    for (auto& x : X) x = u();
+    for (auto& v : y) v = u() > 0.0 ? 1.0 : 0.0;
+    for (auto& v : th) v = 0.3 * u();
+    for (auto& v : r) v = u();
+    EmuGlm e{};
+    e.family = AHMC_GLM_BERNOULLI_LOGIT; e.D = D; e.n = n; e.N = N; e.X = X.data(); e.y = y.data(); e.prec = prec.data();
+    e.eps = 0.05; e.n_steps = steps; e.fwd = 1; e.th_in = th.data(); e.r_in = r.data();
+    double* p = o.data();
+    e.th_out = p; e.r_out = p + N * D; e.g_out = p + 2 * N * D; e.dr_out = p + 3 * N * D; e.lp_out = lp.data(); e.lk_out = lk.data();
+    e.status = status.data(); e.steps_done = done.data();
+    const int rc = emu_glm(&e);
+    int bad = rc != 0;
+    for (int c = 0; c < N; ++c) bad |= status[c] != 0 || done[c] != steps || !std::isfinite(lp[c]);
+    std::printf("glm D %d n %d N %d: rc %d\n", D, n, N, bad);
+    return bad;
+}
 #else
-#error "define RACE_NUTS, RACE_DENSE, RACE_LF, RACE_MN or RACE_ADAPT"
+#error "define RACE_NUTS, RACE_DENSE, RACE_LF, RACE_MN, RACE_ADAPT or RACE_GLM"
 #endif
