@@ -1,8 +1,8 @@
 // adapt_chain_emu.cpp -- runs the two adaptive persistent kernels (K3 adaptive NUTS, ahmc_nuts_kernel.cuh; K2 adaptive
 // static HMC, ahmc_leapfrog.cu; both with the per-chain adaptor of ahmc_chain_adapt.cuh) under the CPU SIMT emulator, on
 // a diagonal Gaussian with the Diag metric and the Philox streams.  The sources are included unmodified (their host launch
-// code is skipped with AHMC_SIMT_EMULATION).  Built with -DADAPT_CHAIN_RACE it is a ThreadSanitizer program of its own
-// (see race_main.cpp for the method).  TEST INFRASTRUCTURE ONLY (tests/test_adapt_in_launch_cpu.py).
+// code is skipped with AHMC_SIMT_EMULATION).  Built with -DRACE_ADAPT_CHAIN it is a ThreadSanitizer program of its own
+// (emu_harness.h describes the method).  TEST INFRASTRUCTURE ONLY (tests/test_adapt_in_launch_cpu.py).
 #define AHMC_SIMT_EMULATION 1
 #include <cstdio>
 #include <cstdlib>
@@ -10,11 +10,11 @@
 
 #include "ahmc_nuts_kernel.cuh"
 #include "ahmc_leapfrog.cu"
+#include "emu_harness.h"
 
 namespace ahmc {
 double smem[1 << 16];  // the block's dynamic shared memory
 }
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 
 using namespace ahmc;
 
@@ -33,6 +33,7 @@ struct EmuAdaptChain {
     int32_t* n_steps_out;             // T x N
     double *eps_rw, *minv_rw;         // N, N x D
 };
+EMU_EXPORT_SIZEOF(EmuAdaptChain);
 
 // FORM: the adaptor's compiled estimator form (adapt_form), as the library's launchers pick it
 template <int G, int E, int FORM>
@@ -109,7 +110,7 @@ extern "C" int emu_adapt_chain(const EmuAdaptChain* q) {
     return 0;
 }
 
-#ifdef ADAPT_CHAIN_RACE
+#ifdef RACE_ADAPT_CHAIN
 static int run(int hmc, int D, int N, int T, int adapt_metric) {
     std::vector<double> mu(D), w(D), Minv(D), th((size_t)N * D), g((size_t)N * D), lp(N, 0.0);
     srand(13 + D);
@@ -144,7 +145,7 @@ static int run(int hmc, int D, int N, int T, int adapt_metric) {
 int main() {
     // N fills its blocks.  In a ragged block the idle groups alias chain N - 1 (`chain = N - 1`): like every persistent
     // kernel of the library they re-read that chain's in-flight state (its phase point, here also its step size) while
-    // its owner group writes it, and discard what they computed -- benign reads, excluded here as in race_main.cpp.
+    // its owner group writes it, and discard what they computed -- benign reads, excluded here as in nuts_emu.cpp's main.
     int bad = 0;
     bad |= run(0, 6, 16, 12, 2);  // NUTS + NutpieVar, four chains per warp
     bad |= run(1, 6, 16, 12, 2);  // static HMC + NutpieVar

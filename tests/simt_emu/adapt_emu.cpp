@@ -2,11 +2,13 @@
 // CPU SIMT emulator (block barriers, static shared variables, the last-block reduction).  TEST INFRASTRUCTURE ONLY.
 #define AHMC_SIMT_EMULATION 1
 #define __shared__ static  // this file's kernels use static shared variables only; blocks run one at a time
+#include <cstdlib>
+#include <cstdio>
 #include <vector>
 
 #include "ahmc_adapt.cu"
+#include "emu_harness.h"
 
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 using namespace ahmc;
 
 struct SumArgs {
@@ -49,3 +51,17 @@ extern "C" int emu_adapt(int D, long long N, const double* theta, const double* 
     emu_launch(cov_thunk, &c, T * (T + 1) / 2, 256);
     return 0;
 }
+
+#ifdef RACE_ADAPT
+int main() {
+    const int D = 37;
+    const long long N = 300;
+    std::vector<double> theta((size_t)N * D), alpha(N), rec(2 + 2 * D), cov((size_t)D * D);
+    srand(2);
+    for (auto& x : theta) x = rand() / (double)RAND_MAX - 0.5;
+    for (auto& x : alpha) x = rand() / (double)RAND_MAX;
+    const int rc = emu_adapt(D, N, theta.data(), alpha.data(), rec.data(), cov.data());
+    std::printf("adapt D %d N %lld: rc %d n %.0f\n", D, N, rc, rec[0]);
+    return rc != 0 || rec[0] != (double)N;
+}
+#endif

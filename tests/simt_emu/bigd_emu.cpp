@@ -1,7 +1,7 @@
 // bigd_emu.cpp -- runs the D > 512 sampling kernels (advancedhmc.jl_b200/csrc/ahmc_bigd_hmc.cu: the static transition,
 // its adaptive form and find_good_stepsize, all on the shared streamed step of ahmc_bigd.cuh) under the CPU SIMT emulator.
-// The source is included unmodified (its host launch code is skipped with AHMC_SIMT_EMULATION).  Built with -DBIGD_RACE it
-// is a ThreadSanitizer program of its own (see race_main.cpp for the method).  TEST INFRASTRUCTURE ONLY
+// The source is included unmodified (its host launch code is skipped with AHMC_SIMT_EMULATION).  Built with -DRACE_BIGD it
+// is a ThreadSanitizer program of its own (emu_harness.h describes the method).  TEST INFRASTRUCTURE ONLY
 // (tests/test_bigd_transitions_cpu.py).
 #define AHMC_SIMT_EMULATION 1
 #include <cmath>
@@ -10,8 +10,7 @@
 #include <vector>
 
 #include "ahmc_bigd_hmc.cu"
-
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
+#include "emu_harness.h"
 
 using namespace ahmc;
 
@@ -36,6 +35,7 @@ struct EmuBigd {
     int32_t adapt_metric, n_adapts, init_buffer, term_buffer, window_size, n_min;
     double *eps_rw, *minv_rw, *eps_trace;
 };
+EMU_EXPORT_SIZEOF(EmuBigd);
 
 template <int MODEL, int METRIC, int ADAPT>
 static void hmc_thunk(const void* p) {
@@ -111,7 +111,7 @@ extern "C" int emu_bigd_find_eps(int32_t model, int32_t metric, int32_t D, int64
     return 0;
 }
 
-#ifdef BIGD_RACE
+#ifdef RACE_BIGD
 // a persistent Philox run of each kernel form on a ragged block (N = 6: two warps of the second block idle)
 static int run(int model, int metric, int adapt_metric, int D, int N, int T) {
     std::vector<double> mu(D), w(D), Minv(D), th((size_t)N * D), r((size_t)N * D, 0.0), g((size_t)N * D), lp(N, 0.0), eps(N, 0.05);

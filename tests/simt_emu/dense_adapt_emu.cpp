@@ -2,8 +2,8 @@
 // emulator: the adaptive NUTS kernel (ahmc_nuts_kernel.cuh) and the adaptive static-HMC kernel (ahmc_leapfrog.cu) on a
 // diagonal Gaussian with a per-chain Dense metric and the Philox streams, and the window-end estimate + Cholesky
 // factorisation on its own, on a workspace the caller fills.  The sources are included unmodified (their host launch code is
-// skipped with AHMC_SIMT_EMULATION).  Built with -DDENSE_ADAPT_RACE it is a ThreadSanitizer program of its own (see
-// race_main.cpp for the method).  TEST INFRASTRUCTURE ONLY (tests/test_dense_adapt_cpu.py).
+// skipped with AHMC_SIMT_EMULATION).  Built with -DRACE_DENSE_ADAPT it is a ThreadSanitizer program of its own
+// (emu_harness.h describes the method).  TEST INFRASTRUCTURE ONLY (tests/test_dense_adapt_cpu.py).
 #define AHMC_SIMT_EMULATION 1
 #include <cmath>
 #include <cstdio>
@@ -12,11 +12,11 @@
 
 #include "ahmc_nuts_kernel.cuh"
 #include "ahmc_leapfrog.cu"
+#include "emu_harness.h"
 
 namespace ahmc {
 double smem[1 << 16];  // the block's dynamic shared memory
 }
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 
 using namespace ahmc;
 
@@ -37,6 +37,7 @@ struct EmuDenseAdapt {
     double *eps_rw, *minv_rw, *cholu_rw;  // N, N x D x D, N x D x D
     double* workspace;                // out: N x (D + D*D), the estimator state (mean, M) after the launch
 };
+EMU_EXPORT_SIZEOF(EmuDenseAdapt);
 
 template <int G, int E>
 static void nuts_thunk(const void* p) {
@@ -126,6 +127,7 @@ struct EmuEstimate {
     double *minv, *cholu;
     int32_t* ok;
 };
+EMU_EXPORT_SIZEOF(EmuEstimate);
 template <int G, int E>
 static void estimate_thunk(const void* p) {
     const EmuEstimate& q = *static_cast<const EmuEstimate*>(p);
@@ -153,7 +155,7 @@ extern "C" int emu_dense_estimate(const EmuEstimate* q) {
     return 0;
 }
 
-#ifdef DENSE_ADAPT_RACE
+#ifdef RACE_DENSE_ADAPT
 static int run(int hmc, int D, int N, int T) {
     std::vector<double> mu(D), w(D), Minv((size_t)N * D * D, 0.0), U((size_t)N * D * D, 0.0), th((size_t)N * D), g((size_t)N * D),
         lp(N, 0.0);
@@ -190,7 +192,7 @@ static int run(int hmc, int D, int N, int T) {
 
 int main() {
     // N fills its blocks (idle groups of a ragged block alias chain N - 1 and re-read its in-flight state: benign reads,
-    // excluded here as in race_main.cpp)
+    // excluded here as in nuts_emu.cpp's main)
     int bad = 0;
     bad |= run(0, 6, 16, 12);  // NUTS, four chains per warp
     bad |= run(1, 7, 16, 12);  // static HMC

@@ -4,14 +4,15 @@
 // TEST INFRASTRUCTURE ONLY (tests/test_simt_emulation.py).
 #define AHMC_SIMT_EMULATION 1
 #define __shared__ static  // static shared variables; blocks run one at a time
+#include <cstdlib>
+#include <cstdio>
 #include <atomic>
 #include <thread>
 #include <vector>
 
 #include "ahmc_dense.cu"
 #include "emu_smem.h"
-
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
+#include "emu_harness.h"
 
 namespace ahmc {
 unsigned char* emu_dynamic_smem = nullptr;
@@ -54,6 +55,7 @@ struct EmuDense {
     int32_t wide_tile;  // RB == 2 only: 1 -> the <2,4> (32-chain) form instead of the default <2,2,2>
     double norms_out[2];
 };
+EMU_EXPORT_SIZEOF(EmuDense);
 
 extern "C" int emu_dense_stages() { return kStages; }
 extern "C" int emu_dense(EmuDense* q) {
@@ -107,3 +109,43 @@ extern "C" int emu_dense(EmuDense* q) {
     emu_dynamic_smem = nullptr;
     return 0;
 }
+
+#ifdef RACE_DENSE
+static int run(int D, int N, bool denseP, bool denseM, int n, int wide) {
+    std::vector<double> P((size_t)D * D, 0.0), M((size_t)D * D, 0.0), w(D), md(D), mu(D, 0.1), th((size_t)N * D), r((size_t)N * D),
+        g((size_t)N * D), o((size_t)4 * N * D), lp(N), lk(N);
+    srand(3 + D);
+    auto u = [] { return rand() / (double)RAND_MAX; };
+    for (int i = 0; i < D; ++i) {
+        P[(size_t)i * D + i] = 1.0 + 0.01 * i;
+        M[(size_t)i * D + i] = 0.5 + 0.002 * i;
+        if (i) P[(size_t)i * D + i - 1] = P[(size_t)(i - 1) * D + i] = 0.1, M[(size_t)i * D + i - 1] = M[(size_t)(i - 1) * D + i] = 0.05;
+        w[i] = 0.8 + 0.4 * u();
+        md[i] = 0.7 + 0.5 * u();
+    }
+    for (auto* v : {&th, &r, &g})
+        for (auto& x : *v) x = u() - 0.5;
+    std::vector<uint32_t> st(N);
+    std::vector<int32_t> done(N);
+    std::vector<uint8_t> need(N);
+    EmuDense q{};
+    q.D = D; q.N = N; q.P = denseP ? P.data() : nullptr; q.w = denseP ? nullptr : w.data(); q.mu = mu.data();
+    q.Minv = denseM ? M.data() : nullptr; q.Mdiag = denseM ? nullptr : md.data(); q.eps = 0.1; q.n_steps = n; q.fwd = 1;
+    q.th_in = th.data(); q.r_in = r.data(); q.g_in = g.data();
+    q.th_out = o.data(); q.r_out = o.data() + (size_t)N * D; q.g_out = o.data() + (size_t)2 * N * D; q.dr_out = o.data() + (size_t)3 * N * D;
+    q.lp_out = lp.data(); q.lk_out = lk.data(); q.status = st.data(); q.steps_done = done.data(); q.need_exact = need.data();
+    q.wide_tile = wide;
+    const int rc = emu_dense(&q);
+    std::printf("dense D %d N %d P %d M %d: rc %d lp0 %.6f need0 %d\n", D, N, (int)denseP, (int)denseM, rc, lp[0], (int)need[0]);
+    return rc != 0 || need[0] != 0;
+}
+
+int main() {
+    int bad = 0;
+    bad |= run(40, 37, true, true, 4, 0);    // <1,4>: two products per step, ragged second tile
+    bad |= run(100, 20, true, false, 3, 0);  // <2,2,2>
+    bad |= run(70, 33, false, true, 3, 1);   // <2,4>
+    bad |= run(130, 9, true, true, 2, 0);    // <3,2>: 12 chunks per product
+    return bad;
+}
+#endif

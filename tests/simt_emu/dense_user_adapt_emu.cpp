@@ -7,7 +7,7 @@
 // P (th - mu), the group sums the shares with ahmc_group_sum), without it the one-lane form.  A shuffle or __syncwarp here
 // is a barrier of all 32 lanes of the warp, so a model call or an estimator exchange that some lane of the warp does not
 // reach would never return.  The sources are included unmodified (their host launch code is skipped with
-// AHMC_SIMT_EMULATION).  Built with -DDENSE_USER_ADAPT_RACE it is a ThreadSanitizer program of its own (race_main.cpp
+// AHMC_SIMT_EMULATION).  Built with -DRACE_DENSE_USER_ADAPT it is a ThreadSanitizer program of its own (emu_harness.h
 // describes the method).  TEST INFRASTRUCTURE ONLY (tests/test_dense_user_adapt_cpu.py).
 #define AHMC_SIMT_EMULATION 1
 #define AHMC_NVRTC_USER_MODEL 1
@@ -21,11 +21,11 @@
 
 #include "ahmc_nuts_kernel.cuh"
 #include "ahmc_leapfrog.cu"
+#include "emu_harness.h"
 
 namespace ahmc {
 double smem[1 << 16];  // the block's dynamic shared memory
 }
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 
 using namespace ahmc;
 
@@ -78,6 +78,7 @@ struct EmuDenseUserAdapt {
     uint8_t *is_accept, *numerical;     // T x N
     double *eps_rw, *minv_rw, *cholu_rw;  // N, N x D x D, N x D x D
 };
+EMU_EXPORT_SIZEOF(EmuDenseUserAdapt);
 
 template <int G, int E>
 static void nuts_thunk(const void* p) {
@@ -156,7 +157,7 @@ extern "C" int emu_dense_user_adapt(const EmuDenseUserAdapt* q) {
     return 0;
 }
 
-#ifdef DENSE_USER_ADAPT_RACE
+#ifdef RACE_DENSE_USER_ADAPT
 static int run(int hmc, int D, int N, int T) {
     std::vector<double> params((size_t)D + (size_t)D * D, 0.0), Minv((size_t)N * D * D, 0.0), U((size_t)N * D * D, 0.0),
         th((size_t)N * D), g((size_t)N * D), lp(N, 0.0);
@@ -205,7 +206,7 @@ static int run(int hmc, int D, int N, int T) {
 
 int main() {
     // N fills its blocks (idle groups of a ragged block alias chain N - 1 and re-read its in-flight state: benign reads,
-    // excluded here as in race_main.cpp)
+    // excluded here as in nuts_emu.cpp's main)
     int bad = 0;
     bad |= run(0, 6, 16, 12);  // NUTS, four chains per warp
     bad |= run(1, 6, 16, 12);  // static HMC

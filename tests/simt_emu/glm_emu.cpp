@@ -3,13 +3,14 @@
 // restated in simt_emu.cpp with the same contracts.  TEST INFRASTRUCTURE ONLY (tests/test_glm_cpu.py).
 #define AHMC_SIMT_EMULATION 1
 #define __shared__ static
+#include <cstdlib>
+#include <cstdio>
 #include <cstring>
 #include <vector>
 
 #include "ahmc_glm.cu"
 #include "emu_smem.h"
-
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
+#include "emu_harness.h"
 
 namespace ahmc {
 unsigned char* emu_dynamic_smem = nullptr;
@@ -36,6 +37,7 @@ struct EmuGlm {
     int32_t* steps_done;
     int32_t nc_out, stages_out;
 };
+EMU_EXPORT_SIZEOF(EmuGlm);
 
 extern "C" int emu_glm(EmuGlm* e) {
     GlmArgs a{};
@@ -66,3 +68,30 @@ extern "C" int emu_glm(EmuGlm* e) {
     emu_dynamic_smem = nullptr;
     return 0;
 }
+
+#ifdef RACE_GLM
+// K6: a 9-coordinate Bernoulli-logit target with 70 rows (two chunks, a partial last one), a ragged second tile
+int main() {
+    const int D = 9, n = 70, N = 17, steps = 2;
+    std::vector<double> X((size_t)n * D), y(n), prec(D, 1.0), th((size_t)N * D), r((size_t)N * D), o((size_t)6 * N * D), lp(N), lk(N);
+    std::vector<uint32_t> status(N);
+    std::vector<int32_t> done(N);
+    srand(3);
+    auto u = [] { return rand() / (double)RAND_MAX - 0.5; };
+    for (auto& x : X) x = u();
+    for (auto& v : y) v = u() > 0.0 ? 1.0 : 0.0;
+    for (auto& v : th) v = 0.3 * u();
+    for (auto& v : r) v = u();
+    EmuGlm e{};
+    e.family = AHMC_GLM_BERNOULLI_LOGIT; e.D = D; e.n = n; e.N = N; e.X = X.data(); e.y = y.data(); e.prec = prec.data();
+    e.eps = 0.05; e.n_steps = steps; e.fwd = 1; e.th_in = th.data(); e.r_in = r.data();
+    double* p = o.data();
+    e.th_out = p; e.r_out = p + N * D; e.g_out = p + 2 * N * D; e.dr_out = p + 3 * N * D; e.lp_out = lp.data(); e.lk_out = lk.data();
+    e.status = status.data(); e.steps_done = done.data();
+    const int rc = emu_glm(&e);
+    int bad = rc != 0;
+    for (int c = 0; c < N; ++c) bad |= status[c] != 0 || done[c] != steps || !std::isfinite(lp[c]);
+    std::printf("glm D %d n %d N %d: rc %d\n", D, n, N, bad);
+    return bad;
+}
+#endif

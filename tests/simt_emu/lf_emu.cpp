@@ -2,13 +2,15 @@
 // advancedhmc.jl_b200/csrc/ahmc_leapfrog.cu + ahmc_traj.cuh, unmodified) under the CPU SIMT emulator.
 // TEST INFRASTRUCTURE ONLY (tests/test_simt_emulation.py).
 #define AHMC_SIMT_EMULATION 1
+#include <cstdlib>
+#include <cstdio>
 #include <vector>
 
 #include "ahmc_leapfrog.cu"
 #include "emu_smem.h"
+#include "emu_harness.h"
 
 EMU_DEFINE_SMEM_ARENA();  // the block's dynamic shared memory (`extern __shared__ double smem[]` in the kernels)
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 using namespace ahmc;
 
 struct EmuLf {
@@ -36,6 +38,7 @@ struct EmuLf {
     double *acc, *dH;
     double* draws;
 };
+EMU_EXPORT_SIZEOF(EmuLf);
 
 template <int MODEL, int METRIC, int G, int E>
 static void lf_thunk(const void* p) { leapfrog_kernel<MODEL, METRIC, G, E>(*static_cast<const LeapfrogArgs*>(p)); }
@@ -107,3 +110,70 @@ extern "C" int emu_leapfrog(const EmuLf* q) {
     emu_smem_end();
     return 0;
 }
+
+#ifdef RACE_LF
+static int run(int model, int metric, int D, int N, int n, int hmc) {
+    std::vector<double> mu(D), w(D), P, Minv, cholU, th((size_t)N * D), r((size_t)N * D), g((size_t)N * D), lp(N, 0.0);
+    srand(5 + D);
+    auto u = [] { return rand() / (double)RAND_MAX; };
+    for (int d = 0; d < D; ++d) mu[d] = u() - 0.5, w[d] = 0.5 + u();
+    if (model == AHMC_MODEL_DENSE_GAUSS) {
+        P.assign((size_t)D * D, 0.0);
+        for (int d = 0; d < D; ++d) {
+            P[(size_t)d * D + d] = 1.0 + 0.1 * u();
+            if (d) P[(size_t)d * D + d - 1] = P[(size_t)(d - 1) * D + d] = 0.2;
+        }
+    }
+    if (metric == AHMC_METRIC_DIAG) {
+        Minv.resize(D);
+        for (auto& x : Minv) x = 0.7 + 0.6 * u();
+    } else if (metric == AHMC_METRIC_DENSE) {
+        Minv.assign((size_t)D * D, 0.0);
+        cholU.assign((size_t)D * D, 0.0);
+        for (int d = 0; d < D; ++d) {
+            const double s = 0.8 + 0.4 * u();
+            Minv[(size_t)d * D + d] = s * s;
+            cholU[(size_t)d * D + d] = s;
+        }
+    }
+    for (int c = 0; c < N; ++c)
+        for (int d = 0; d < D; ++d) {
+            th[(size_t)c * D + d] = u() - 0.5;
+            r[(size_t)c * D + d] = u() - 0.5;
+        }
+    for (int c = 0; c < N; ++c)
+        for (int d = 0; d < D; ++d) {
+            double gd = 0.0;
+            if (model == AHMC_MODEL_DENSE_GAUSS)
+                for (int k = 0; k < D; ++k) gd += P[(size_t)k * D + d] * (th[(size_t)c * D + k] - mu[k]);
+            else gd = (th[(size_t)c * D + d] - mu[d]) * w[d];
+            g[(size_t)c * D + d] = gd;
+            lp[c] -= 0.5 * gd * (th[(size_t)c * D + d] - mu[d]);
+        }
+    std::vector<double> o((size_t)4 * N * D), lpo(N), lko(N), acc(N), dH(N);
+    std::vector<uint32_t> st(N);
+    std::vector<int32_t> done(N);
+    std::vector<uint8_t> isacc(N);
+    EmuLf q{};
+    q.model_kind = model; q.metric_kind = metric; q.D = D; q.N = N; q.p0 = mu.data();
+    q.p1 = model == AHMC_MODEL_DENSE_GAUSS ? P.data() : w.data();
+    q.Minv = Minv.data(); q.cholU = cholU.empty() ? nullptr : cholU.data(); q.eps = 0.1; q.n_steps = n; q.fwd = 1;
+    q.th_in = th.data(); q.r_in = r.data(); q.g_in = g.data(); q.lp_in = lp.data();
+    q.th_out = o.data(); q.r_out = o.data() + (size_t)N * D; q.g_out = o.data() + (size_t)2 * N * D; q.dr_out = o.data() + (size_t)3 * N * D;
+    q.lp_out = lpo.data(); q.lk_out = lko.data(); q.status = st.data(); q.steps_done = done.data();
+    q.hmc = hmc; q.refresh = 1; q.n_transitions = 1; q.seed = 3; q.is_accept = isacc.data(); q.acc = acc.data(); q.dH = dH.data();
+    const int rc = emu_leapfrog(&q);
+    std::printf("lf model %d metric %d D %d N %d hmc %d: rc %d lp0 %.6f\n", model, metric, D, N, hmc, rc, lpo[0]);
+    return rc != 0;
+}
+
+int main() {
+    int bad = 0;
+    bad |= run(AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, 7, 21, 12, 0);   // K1 fused fast path, four chains per warp, ragged block
+    bad |= run(AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE, 6, 9, 6, 0);   // K1 exact path with the shared-memory operator slabs
+    bad |= run(AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, 40, 5, 8, 0);    // one chain per warp
+    bad |= run(AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, 7, 21, 5, 1);    // K2: refresh + trajectory + Metropolis step
+    bad |= run(AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE, 6, 9, 4, 1);
+    return bad;
+}
+#endif

@@ -1,14 +1,16 @@
 // mn_emu.cpp -- the MultinomialTS static-transition kernel (advancedhmc.jl_b200/csrc/ahmc_multinomial.cu, unmodified)
 // under the CPU SIMT emulator.  TEST INFRASTRUCTURE ONLY (tests/test_simt_emulation.py).
 #define AHMC_SIMT_EMULATION 1
+#include <cstdlib>
+#include <cstdio>
 #include <vector>
 
 #include "ahmc_multinomial.cu"
+#include "emu_harness.h"
 
 namespace ahmc {
 double smem[1 << 16];
 }
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 using namespace ahmc;
 
 struct EmuMn {
@@ -26,6 +28,7 @@ struct EmuMn {
     int32_t* index;
     double temper_alpha;
 };
+EMU_EXPORT_SIZEOF(EmuMn);
 
 template <int MODEL, int METRIC, int G, int E>
 static void mn_thunk(const void* p) { multinomial_kernel<MODEL, METRIC, G, E>(*static_cast<const MultinomialArgs*>(p)); }
@@ -74,3 +77,57 @@ extern "C" int emu_multinomial(const EmuMn* q) {
     emu_launch(fn, &a, (int)((q->N + chains_per_block - 1) / chains_per_block), kBlockThreads);
     return 0;
 }
+
+#ifdef RACE_MN
+static int run(int model, int metric, int D, int N, int n, int n_fwd) {
+    std::vector<double> mu(D), w(D), P, Minv, cholU, th((size_t)N * D), g((size_t)N * D), lp(N, 0.0);
+    std::vector<double> normals((size_t)N * D), unif(N);
+    srand(9 + D);
+    auto u = [] { return rand() / (double)RAND_MAX; };
+    for (int d = 0; d < D; ++d) mu[d] = u() - 0.5, w[d] = 0.5 + u();
+    if (model == AHMC_MODEL_DENSE_GAUSS) {
+        P.assign((size_t)D * D, 0.0);
+        for (int d = 0; d < D; ++d) {
+            P[(size_t)d * D + d] = 1.0 + 0.1 * u();
+            if (d) P[(size_t)d * D + d - 1] = P[(size_t)(d - 1) * D + d] = 0.2;
+        }
+    }
+    if (metric == AHMC_METRIC_DIAG) {
+        Minv.resize(D);
+        for (auto& x : Minv) x = 0.7 + 0.6 * u();
+    }
+    for (int c = 0; c < N; ++c) {
+        unif[c] = u();
+        for (int d = 0; d < D; ++d) th[(size_t)c * D + d] = u() - 0.5, normals[(size_t)c * D + d] = 2.0 * u() - 1.0;
+    }
+    for (int c = 0; c < N; ++c)
+        for (int d = 0; d < D; ++d) {
+            double gd = 0.0;
+            if (model == AHMC_MODEL_DENSE_GAUSS)
+                for (int k = 0; k < D; ++k) gd += P[(size_t)k * D + d] * (th[(size_t)c * D + k] - mu[k]);
+            else gd = (th[(size_t)c * D + d] - mu[d]) * w[d];
+            g[(size_t)c * D + d] = gd;
+            lp[c] -= 0.5 * gd * (th[(size_t)c * D + d] - mu[d]);
+        }
+    std::vector<double> o((size_t)3 * N * D), lpo(N), lko(N), acc(N);
+    std::vector<int32_t> idx(N);
+    EmuMn q{};
+    q.model_kind = model; q.metric_kind = metric; q.D = D; q.N = N; q.p0 = mu.data();
+    q.p1 = model == AHMC_MODEL_DENSE_GAUSS ? P.data() : w.data();
+    q.Minv = Minv.empty() ? nullptr : Minv.data(); q.eps = 0.2; q.n_steps = n; q.n_fwd = n_fwd;
+    q.normal_tape = normals.data(); q.unif_tape = unif.data(); q.th_in = th.data(); q.g_in = g.data(); q.lp_in = lp.data();
+    q.th_out = o.data(); q.r_out = o.data() + (size_t)N * D; q.g_out = o.data() + (size_t)2 * N * D;
+    q.lp_out = lpo.data(); q.lk_out = lko.data(); q.acc = acc.data(); q.index = idx.data();
+    const int rc = emu_multinomial(&q);
+    std::printf("mn model %d metric %d D %d N %d: rc %d acc0 %.6f\n", model, metric, D, N, rc, acc[0]);
+    return rc != 0;
+}
+
+int main() {
+    int bad = 0;
+    bad |= run(AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, 7, 21, 7, 3);    // four chains per warp, ragged block, both directions
+    bad |= run(AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_UNIT, 6, 9, 5, 5);    // shared-memory precision slab
+    bad |= run(AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, 40, 5, 6, 0);    // one chain per warp, all backward
+    return bad;
+}
+#endif

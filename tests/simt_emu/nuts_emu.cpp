@@ -2,14 +2,15 @@
 // TEST INFRASTRUCTURE ONLY: built by tests/test_simt_emulation.py with g++; the kernel header is included unmodified
 // (its host launch code is skipped with AHMC_SIMT_EMULATION).
 #define AHMC_SIMT_EMULATION 1
+#include <cstdio>
 #include <cstdlib>
 #include <vector>
 
 #include "ahmc_nuts_kernel.cuh"
 #include "emu_smem.h"
+#include "emu_harness.h"
 
 EMU_DEFINE_SMEM_ARENA();  // the block's dynamic shared memory (`extern __shared__ double smem[]` in the kernel)
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 
 using namespace ahmc;
 
@@ -47,6 +48,7 @@ struct EmuNuts {
     double temper_alpha;
     int32_t coop_padded;  // 1: also hand the kernel column-padded copies of the dense matrices (one bulk copy per chunk)
 };
+EMU_EXPORT_SIZEOF(EmuNuts);
 
 template <int MODEL, int METRIC, int G, int E, bool VAR, bool ADAPT>
 static constexpr bool coop_form() {  // like launch_nuts_v: dense operators, one chain per warp, default family
@@ -207,3 +209,87 @@ extern "C" int emu_nuts(const EmuNuts* q) {
     emu_smem_end();
     return 0;
 }
+
+#ifdef RACE_NUTS
+static int run(int model, int metric, int D, int N, int T, int sampler, int criterion, bool adapt) {
+    std::vector<double> mu(D), w(D), Minv, cholU, th((size_t)N * D), r((size_t)N * D, 0.0), g((size_t)N * D), lp(N, 0.0);
+    std::vector<double> P;
+    srand(7 + D);
+    auto u = [] { return rand() / (double)RAND_MAX; };
+    for (int d = 0; d < D; ++d) mu[d] = u() - 0.5, w[d] = 0.5 + u();
+    if (model == AHMC_MODEL_DENSE_GAUSS) {  // tridiagonal precision
+        P.assign((size_t)D * D, 0.0);
+        for (int d = 0; d < D; ++d) {
+            P[(size_t)d * D + d] = 1.0 + 0.1 * u();
+            if (d) P[(size_t)d * D + d - 1] = P[(size_t)(d - 1) * D + d] = 0.2;
+        }
+    }
+    if (metric == AHMC_METRIC_DIAG) {
+        Minv.resize(D);
+        for (auto& x : Minv) x = 0.7 + 0.6 * u();
+    } else if (metric == AHMC_METRIC_DENSE) {  // diagonal matrices in dense storage: Minv and its Cholesky factor
+        Minv.assign((size_t)D * D, 0.0);
+        cholU.assign((size_t)D * D, 0.0);
+        for (int d = 0; d < D; ++d) {
+            const double s = 0.8 + 0.4 * u();
+            Minv[(size_t)d * D + d] = s * s;
+            cholU[(size_t)d * D + d] = s;
+        }
+    }
+    for (int c = 0; c < N; ++c) {
+        for (int d = 0; d < D; ++d) th[(size_t)c * D + d] = u() - 0.5;
+        for (int d = 0; d < D; ++d) {  // -grad log pi and log pi at theta
+            double gd = 0.0;
+            if (model == AHMC_MODEL_DENSE_GAUSS)
+                for (int k = 0; k < D; ++k) gd += P[(size_t)k * D + d] * (th[(size_t)c * D + k] - mu[k]);
+            else if (model == AHMC_MODEL_DIAG_GAUSS) gd = (th[(size_t)c * D + d] - mu[d]) * w[d];
+            else gd = th[(size_t)c * D + d];
+            g[(size_t)c * D + d] = gd;
+            lp[c] -= 0.5 * gd * (th[(size_t)c * D + d] - (model == AHMC_MODEL_STD_NORMAL ? 0.0 : mu[d]));
+        }
+    }
+    std::vector<double> o((size_t)3 * N * D), lpo(N), lko(N), acc((size_t)T * N), dH((size_t)T * N), dHm((size_t)T * N);
+    std::vector<double> draws((size_t)T * N * D), eps_rw(N, 0.3), minv_rw((size_t)N * D, 0.0), trace((size_t)T * N);
+    std::vector<int32_t> ns((size_t)T * N), td((size_t)T * N);
+    std::vector<uint8_t> ne((size_t)T * N);
+    EmuNuts q{};
+    q.model_kind = model; q.metric_kind = metric; q.D = D; q.N = N;
+    q.p0 = model == AHMC_MODEL_STD_NORMAL ? nullptr : mu.data();
+    q.p1 = model == AHMC_MODEL_DENSE_GAUSS ? P.data() : (model == AHMC_MODEL_DIAG_GAUSS ? w.data() : nullptr);
+    q.Minv = Minv.empty() ? nullptr : Minv.data();
+    q.cholU = cholU.empty() ? nullptr : cholU.data();
+    q.eps = 0.3; q.max_depth = 5; q.delta_max = 1000.0; q.sampler = sampler; q.criterion = criterion;
+    q.seed = 11; q.refresh = 1;
+    q.th_in = th.data(); q.r_in = r.data(); q.g_in = g.data(); q.lp_in = lp.data();
+    q.th_out = o.data(); q.r_out = o.data() + (size_t)N * D; q.g_out = o.data() + (size_t)2 * N * D;
+    q.lp_out = lpo.data(); q.lk_out = lko.data(); q.n_steps = ns.data(); q.tree_depth = td.data(); q.numerical = ne.data();
+    q.acc = acc.data(); q.dH = dH.data(); q.dHmax = dHm.data(); q.n_transitions = T; q.draws = draws.data();
+    if (adapt) {
+        q.adapt = 1; q.n_adapts = T - 2; q.init_buffer = 2; q.term_buffer = 2; q.window_size = 3;
+        q.delta = 0.8; q.gamma = 0.05; q.t0 = 10.0; q.kappa = 0.75; q.adapt_metric = 1; q.n_min = 3;
+        q.eps_rw = eps_rw.data(); q.minv_rw = minv_rw.data(); q.eps_trace = trace.data();
+    }
+    const int rc = emu_nuts(&q);
+    long steps = 0;
+    for (auto s : ns) steps += s;
+    std::printf("nuts model %d metric %d D %d N %d sampler %d criterion %d adapt %d: rc %d, %ld leapfrog steps\n", model, metric, D, N,
+                sampler, criterion, (int)adapt, rc, steps);
+    return rc != 0 || steps < (long)T * N;
+}
+
+int main() {
+    int bad = 0;
+    bad |= run(AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, 6, 9, 4, 0, 0, false);    // four chains per warp, ragged last block
+    bad |= run(AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, 40, 5, 3, 0, 0, false);   // one chain per warp (or the alt layouts)
+    bad |= run(AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, 100, 3, 2, 0, 0, false);  // the headline layout
+    bad |= run(AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE, 6, 5, 3, 0, 0, false);  // shared-memory operator slabs
+    bad |= run(AHMC_MODEL_FUNNEL, AHMC_METRIC_DIAG, 5, 6, 3, 1, 2, false);        // SliceTS + strict criterion family
+    bad |= run(AHMC_MODEL_STD_NORMAL, AHMC_METRIC_UNIT, 3, 7, 3, 0, 1, false);    // classic criterion
+    bad |= run(AHMC_MODEL_DENSE_GAUSS, AHMC_METRIC_DENSE, 40, 11, 2, 0, 0, false);  // COOP form: 8 chains per block share the D x D products
+    // in-launch adaptation (chain workspace).  N fills its block: the idle groups of a ragged block alias the LAST chain
+    // read-only (`chain = N - 1`, ahmc_nuts_kernel.cuh) and their unused load of its step size would be reported against the
+    // owner's write-back of the adapted value -- a benign read, excluded here rather than suppressed.
+    bad |= run(AHMC_MODEL_DIAG_GAUSS, AHMC_METRIC_DIAG, 6, 16, 12, 0, 0, true);
+    return bad;
+}
+#endif

@@ -1,7 +1,7 @@
 // pair_emu.cpp -- runs K1's two-chains-per-warp fast path (leapfrog_pair_kernel, ahmc_leapfrog.cu, unmodified) under the
 // CPU SIMT emulator, launched as the product's launcher does for a lane-contiguous full tile: 8 chains per 128-thread
 // block, one coefficient set for the pair when eps is a scalar and M^-1 is shared.  Built alone (tests/test_leapfrog_pair.py)
-// or with -DPAIR_RACE_MAIN -fsanitize=thread as a data-race check of the kernel source.  TEST INFRASTRUCTURE ONLY.
+// or with -DRACE_PAIR -fsanitize=thread as a data-race check of the kernel source.  TEST INFRASTRUCTURE ONLY.
 #include <cstdio>
 #include <cstdlib>
 
@@ -43,7 +43,7 @@ extern "C" int emu_leapfrog_pair(const EmuLf* q) {
     return 0;
 }
 
-#ifdef PAIR_RACE_MAIN
+#ifdef RACE_PAIR
 // N = 11: a ragged last block and a last warp whose B shadows chain 10; chain 4 defeats the magnitude proof (its pair
 // partner stays fast), so the exact path runs inside the same warps.  Shared coefficients, then per-chain eps.
 static int run(bool chain_eps) {

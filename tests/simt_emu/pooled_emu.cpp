@@ -7,8 +7,8 @@
 #include <vector>
 
 #include "ahmc_pooled.cu"
+#include "emu_harness.h"
 
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 using namespace ahmc;
 
 struct UpdArgs {
@@ -24,7 +24,7 @@ static void upd_thunk(const void* p) {
     pooled_update_kernel(a.st, a.gathered, a.R, a.D, a.w_mu, a.w_M2, a.Minv, a.eps_chain, a.N, a.trace, a.merged);
 }
 
-struct EmuPooled {
+struct PooledHandle {
     std::vector<char> state;
     std::vector<double> w_mu, w_M2, Minv, eps_chain, merged;
     int D;
@@ -35,7 +35,7 @@ extern "C" void* emu_pooled_create(int D, long long N, int n_adapts, int init_bu
                                    double delta, int adapt_metric, int n_min) {
     AdaptDev sched{};
     if (!stan_window_schedule(sched, init_buffer, term_buffer, window_size, n_adapts)) return nullptr;
-    EmuPooled* e = new EmuPooled;
+    PooledHandle* e = new PooledHandle;
     e->D = D;
     e->N = N;
     e->state.resize(pooled_state_bytes());
@@ -49,7 +49,7 @@ extern "C" void* emu_pooled_create(int D, long long N, int n_adapts, int init_bu
 }
 // one exchange: `gathered` = R records of (2 + 2D) doubles in rank order
 extern "C" int emu_pooled_update(void* h, const double* gathered, int R, double* eps_out, double* minv_out, double* merged_out) {
-    EmuPooled* e = static_cast<EmuPooled*>(h);
+    PooledHandle* e = static_cast<PooledHandle*>(h);
     UpdArgs a{reinterpret_cast<PooledState*>(e->state.data()), gathered, R, e->D, e->w_mu.data(), e->w_M2.data(), e->Minv.data(),
               e->eps_chain.data(), e->N, nullptr, e->merged.data()};
     emu_launch(upd_thunk, &a, 1, 256);
@@ -61,4 +61,4 @@ extern "C" int emu_pooled_update(void* h, const double* gathered, int R, double*
         if (e->eps_chain[c] != *eps_out) return -1;
     return it;
 }
-extern "C" void emu_pooled_destroy(void* h) { delete static_cast<EmuPooled*>(h); }
+extern "C" void emu_pooled_destroy(void* h) { delete static_cast<PooledHandle*>(h); }

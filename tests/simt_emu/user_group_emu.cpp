@@ -11,11 +11,11 @@
 
 #include "ahmc_leapfrog.cu"
 #include "ahmc_nuts_kernel.cuh"
+#include "emu_harness.h"
 
 namespace ahmc {
 double smem[1 << 16];
 }
-void emu_launch(void (*kernel)(const void*), const void* args, int blocks, int threads);
 using namespace ahmc;
 
 // the user's source (the funnel tests/test_user_group_cpu.py compiles with NVRTC): lane 0 broadcasts e^-v, lane l of the
@@ -57,6 +57,7 @@ struct EmuUser {
     uint8_t* numerical;
     double* acc;
 };
+EMU_EXPORT_SIZEOF(EmuUser);
 
 template <int M, int G, int E>
 static void pp_thunk(const void* p) { phasepoint_kernel<AHMC_MODEL_USER, M, G, E>(*static_cast<const PhasepointArgs*>(p)); }

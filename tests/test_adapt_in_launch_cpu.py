@@ -5,41 +5,18 @@ composed oracle NutpieVar against the 50-digit fixture.  The GPU side is tests/t
 import ctypes as C
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import oracle_c as oc
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU = os.path.join(ROOT, "tests", "simt_emu")
-CSRC = os.path.join(ROOT, "advancedhmc.jl_b200", "csrc")
-_vp = C.c_void_p
-P = lambda a: None if a is None else a.ctypes.data_as(_vp)
-
-
-class EmuAdaptChain(C.Structure):
-    _fields_ = [("hmc", C.c_int32), ("D", C.c_int32), ("N", C.c_int64), ("mu", _vp), ("w", _vp), ("Minv", _vp), ("eps0", C.c_double),
-                ("max_depth", C.c_int32), ("n_steps", C.c_int32), ("seed", C.c_uint64), ("T", C.c_int32), ("n_adapts", C.c_int32),
-                ("init_buffer", C.c_int32), ("term_buffer", C.c_int32), ("window_size", C.c_int32), ("adapt_metric", C.c_int32),
-                ("n_min", C.c_int32), ("th_in", _vp), ("g_in", _vp), ("lp_in", _vp), ("th_out", _vp), ("r_out", _vp), ("g_out", _vp),
-                ("lp_out", _vp), ("lk_out", _vp), ("draws", _vp), ("acc", _vp), ("eps_trace", _vp), ("n_steps_out", _vp),
-                ("eps_rw", _vp), ("minv_rw", _vp)]
-
-
-def _gxx(out, *extra):
-    return ["g++", *extra, "-std=c++20", "-pthread", "-ffp-contract=off", "-w", "-I", os.path.join(EMU, "include"), "-I", CSRC,
-            "-I", os.path.join(ROOT, "include"), os.path.join(EMU, "simt_emu.cpp"), os.path.join(EMU, "adapt_chain_emu.cpp"),
-            "-o", str(out)]
+from tests import emu as E
+from tests.emu import P, EmuAdaptChain
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    out = tmp_path_factory.mktemp("simt_adapt_chain") / "libadapt_chain_emu.so"
-    pr = subprocess.run(_gxx(out, "-O1", "-shared", "-fPIC"), capture_output=True, text=True)
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    return C.CDLL(str(out))
+def emu():
+    return E.harness("adapt_chain")
 
 
 def _run(lib, hmc, est, D, N, T, n_adapts, windows, n_min, seed):
@@ -102,15 +79,8 @@ def test_adaptive_kernel_sources_under_emulation_equal_oracle_adaptors(emu, kern
     assert (run["n_steps"] >= 1).all() and len(np.unique(run["trace"][-1])) == N  # every chain adapted on its own
 
 
-def test_adaptive_kernel_sources_are_data_race_free_under_thread_sanitizer(tmp_path):
-    out = tmp_path / "race_adapt_chain"
-    pr = subprocess.run(_gxx(out, "-DADAPT_CHAIN_RACE", "-O1", "-g", "-fsanitize=thread", "-x", "c++"), capture_output=True, text=True)
-    if pr.returncode != 0 and "tsan" in pr.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available to g++ here")
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    r = subprocess.run([str(out)], capture_output=True, text=True, timeout=900)
-    if "FATAL: ThreadSanitizer" in r.stderr:
-        pytest.skip("ThreadSanitizer cannot run in this environment: " + r.stderr.strip().splitlines()[0])
+def test_adaptive_kernel_sources_are_data_race_free_under_thread_sanitizer():
+    r = E.sanitized("adapt_chain", "thread")
     assert r.returncode == 0 and "WARNING: ThreadSanitizer" not in r.stderr, r.stdout + r.stderr[-3000:]
     assert r.stdout.count("rc 0") == 6, r.stdout
 
@@ -120,29 +90,27 @@ def test_adaptive_user_target_kernels_compile_under_nvrtc():
     Diag metrics, several layouts; a broken source comes back as the NVRTC log"""
     import ahmc_b200 as A
 
-    lib = A._lib.load()
+    lib = E.nvrtc_lib_or_skip()
     general = ("__device__ double ahmc_user_logp_grad(const double* th, double* g, int D, const double* p) {\n"
                "  double s = 0.0; for (int i = 0; i < D; ++i) { g[i] = -th[i] * p[0]; s += th[i] * th[i]; } return -0.5 * p[0] * s; }\n")
     coord = ("#define AHMC_USER_COORDWISE\n__device__ double ahmc_user_coord(int d, double x, const double* p, double* gd) {\n"
              "  *gd = -x * p[d]; return -0.5 * x * x * p[d]; }\n")
-    log = C.create_string_buffer(4096)
-    if lib.ahmc_user_source_check(general.encode(), 5, 1, 8, log, 4096) == A._lib.ERR_UNSUPPORTED:
-        pytest.skip("libnvrtc not available here: " + log.value.decode())
     for src in (general, coord):
         for kernel in (5, 6):
             for metric, D in ((0, 6), (1, 8), (1, 40), (1, 128), (0, 200)):
-                assert lib.ahmc_user_source_check(src.encode(), kernel, metric, D, log, 4096) == 0, log.value.decode()
-    bad = b"__device__ double ahmc_user_logp_grad(const double* t, double* g, int D, const double* p) { return q; }"
+                rc, log = E.source_check(lib, src, kernel, metric, D)
+                assert rc == 0, log
+    bad = "__device__ double ahmc_user_logp_grad(const double* t, double* g, int D, const double* p) { return q; }"
     for kernel in (5, 6):
-        assert lib.ahmc_user_source_check(bad, kernel, 1, 8, log, 4096) == A._lib.ERR_INVALID
-        assert b"q" in log.value and b"undefined" in log.value
-    assert lib.ahmc_user_source_check(general.encode(), 7, 1, 8, log, 4096) == A._lib.ERR_INVALID
+        rc, log = E.source_check(lib, bad, kernel, 1, 8)
+        assert rc == A._lib.ERR_INVALID and "q" in log and "undefined" in log
+    assert E.source_check(lib, general, 7, 1, 8)[0] == A._lib.ERR_INVALID
 
 
 def test_composed_oracle_nutpie_var_reproduces_the_50_digit_fixture():
     """NutpieVar as the kernels build it -- two WelfordVar of positions and (minus) gradients, M^-1 = sqrt(est / est) --
     composed from the oracle's WelfordVar, against tests/golden/adapt_mp50.json"""
-    with open(os.path.join(ROOT, "tests", "golden", "adapt_mp50.json")) as f:
+    with open(os.path.join(E.ROOT, "tests", "golden", "adapt_mp50.json")) as f:
         w = json.load(f)["welford"]
     xs, gs = np.array(w["xs"]), np.array(w["gs"])
     for sign in (1.0, -1.0):  # the kernels push MINUS grad log pi: the same variance

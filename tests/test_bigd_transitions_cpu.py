@@ -3,46 +3,22 @@ tape-driven static transitions against the ORACLE, a persistent run against sing
 replayed against the oracle's adaptors, find_good_stepsize against the search restated on the oracle's leapfrog, and
 the same sources under ThreadSanitizer.  The GPU side is tests/test_bigd_transitions.py."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import oracle_c as oc
+from tests import emu as E
+from tests.emu import P, EmuBigd
 from tests.helpers import rel_err
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU = os.path.join(ROOT, "tests", "simt_emu")
-CSRC = os.path.join(ROOT, "advancedhmc.jl_b200", "csrc")
-_vp = C.c_void_p
-P = lambda a: None if a is None else a.ctypes.data_as(_vp)
 UNIT, DIAG = 0, 1
 MODELS = {"std_normal": oc.STD_NORMAL, "diag_gauss": oc.DIAG_GAUSS, "funnel": oc.FUNNEL}
 
 
-class EmuBigd(C.Structure):
-    _fields_ = [("model", C.c_int32), ("metric", C.c_int32), ("D", C.c_int32), ("N", C.c_int64), ("p0", _vp), ("p1", _vp),
-                ("c0", C.c_double), ("Minv", _vp), ("minv_stride", C.c_int64), ("eps", _vp), ("n_steps", C.c_int32), ("T", C.c_int32),
-                ("refresh", C.c_int32), ("seed", C.c_uint64), ("offset", C.c_uint64), ("partial_alpha", C.c_double), ("normal_tape", _vp), ("exp_tape", _vp),
-                ("th_in", _vp), ("r_in", _vp), ("g_in", _vp), ("lp_in", _vp), ("th_out", _vp), ("r_out", _vp), ("g_out", _vp),
-                ("lp_out", _vp), ("lk_out", _vp), ("draws", _vp), ("acc", _vp), ("H", _vp), ("dH", _vp), ("is_accept", _vp),
-                ("numerical_error", _vp), ("adapt_metric", C.c_int32), ("n_adapts", C.c_int32), ("init_buffer", C.c_int32),
-                ("term_buffer", C.c_int32), ("window_size", C.c_int32), ("n_min", C.c_int32), ("eps_rw", _vp), ("minv_rw", _vp),
-                ("eps_trace", _vp)]
-
-
-def _gxx(out, *extra):
-    return ["g++", *extra, "-std=c++20", "-pthread", "-ffp-contract=off", "-w", "-I", os.path.join(EMU, "include"), "-I", CSRC,
-            "-I", os.path.join(ROOT, "include"), os.path.join(EMU, "simt_emu.cpp"), os.path.join(EMU, "bigd_emu.cpp"), "-o", str(out)]
-
-
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    out = tmp_path_factory.mktemp("simt_bigd") / "libbigd_emu.so"
-    pr = subprocess.run(_gxx(out, "-O1", "-shared", "-fPIC"), capture_output=True, text=True)
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    return C.CDLL(str(out))
+def emu():
+    return E.harness("bigd")
 
 
 class _Problem:
@@ -210,14 +186,7 @@ def test_find_good_stepsize_source_equals_the_search_on_the_oracle(emu):
         assert eps_out[c] == pytest.approx(e, rel=1e-12), c
 
 
-def test_streamed_sampling_sources_are_data_race_free_under_thread_sanitizer(tmp_path):
-    out = tmp_path / "race_bigd"
-    pr = subprocess.run(_gxx(out, "-DBIGD_RACE", "-O1", "-g", "-fsanitize=thread", "-x", "c++"), capture_output=True, text=True)
-    if pr.returncode != 0 and "tsan" in pr.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available to g++ here")
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    r = subprocess.run([str(out)], capture_output=True, text=True, timeout=900)
-    if "FATAL: ThreadSanitizer" in r.stderr:
-        pytest.skip("ThreadSanitizer cannot run in this environment: " + r.stderr.strip().splitlines()[0])
+def test_streamed_sampling_sources_are_data_race_free_under_thread_sanitizer():
+    r = E.sanitized("bigd", "thread")
     assert r.returncode == 0 and "WARNING: ThreadSanitizer" not in r.stderr, r.stdout + r.stderr[-3000:]
     assert r.stdout.count("rc 0 0") == 4, r.stdout

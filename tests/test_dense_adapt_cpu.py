@@ -4,47 +4,20 @@ oracle's DualAveraging and one WelfordCov per chain, the window-end estimate and
 (including a failing factorisation), and the same sources under ThreadSanitizer.  The GPU side is
 tests/test_dense_per_chain.py."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import oracle_c as oc
+from tests import emu as E
+from tests.emu import P, EmuDenseAdapt, EmuEstimate
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU = os.path.join(ROOT, "tests", "simt_emu")
-CSRC = os.path.join(ROOT, "advancedhmc.jl_b200", "csrc")
-_vp = C.c_void_p
-P = lambda a: None if a is None else a.ctypes.data_as(_vp)
 WELFORD_COV = 3
 
 
-class EmuDenseAdapt(C.Structure):
-    _fields_ = [("hmc", C.c_int32), ("D", C.c_int32), ("N", C.c_int64), ("mu", _vp), ("w", _vp), ("Minv0", _vp), ("cholU0", _vp),
-                ("eps0", C.c_double), ("max_depth", C.c_int32), ("n_steps", C.c_int32), ("seed", C.c_uint64), ("T", C.c_int32),
-                ("n_adapts", C.c_int32), ("init_buffer", C.c_int32), ("term_buffer", C.c_int32), ("window_size", C.c_int32),
-                ("adapt_metric", C.c_int32), ("n_min", C.c_int32), ("th_in", _vp), ("g_in", _vp), ("lp_in", _vp), ("th_out", _vp),
-                ("r_out", _vp), ("g_out", _vp), ("lp_out", _vp), ("lk_out", _vp), ("draws", _vp), ("acc", _vp), ("eps_trace", _vp),
-                ("n_steps_out", _vp), ("eps_rw", _vp), ("minv_rw", _vp), ("cholu_rw", _vp), ("workspace", _vp)]
-
-
-class EmuEstimate(C.Structure):
-    _fields_ = [("D", C.c_int32), ("N", C.c_int64), ("n", C.c_double), ("W", _vp), ("minv", _vp), ("cholu", _vp), ("ok", _vp)]
-
-
-def _gxx(out, *extra):
-    return ["g++", *extra, "-std=c++20", "-pthread", "-ffp-contract=off", "-w", "-I", os.path.join(EMU, "include"), "-I", CSRC,
-            "-I", os.path.join(ROOT, "include"), os.path.join(EMU, "simt_emu.cpp"), os.path.join(EMU, "dense_adapt_emu.cpp"),
-            "-o", str(out)]
-
-
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    out = tmp_path_factory.mktemp("simt_dense_adapt") / "libdense_adapt_emu.so"
-    pr = subprocess.run(_gxx(out, "-O1", "-shared", "-fPIC"), capture_output=True, text=True)
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    return C.CDLL(str(out))
+def emu():
+    return E.harness("dense_adapt")
 
 
 def _spd(rng, D, scale=1.0):
@@ -177,14 +150,7 @@ def test_window_end_estimate_and_factor_and_a_failed_factorisation(emu, D, N):
             assert (np.tril(got_U[c], -1) == 0).all()
 
 
-def test_welford_cov_kernel_sources_are_data_race_free_under_thread_sanitizer(tmp_path):
-    out = tmp_path / "race_dense_adapt"
-    pr = subprocess.run(_gxx(out, "-DDENSE_ADAPT_RACE", "-O1", "-g", "-fsanitize=thread", "-x", "c++"), capture_output=True, text=True)
-    if pr.returncode != 0 and "tsan" in pr.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available to g++ here")
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    r = subprocess.run([str(out)], capture_output=True, text=True, timeout=900)
-    if "FATAL: ThreadSanitizer" in r.stderr:
-        pytest.skip("ThreadSanitizer cannot run in this environment: " + r.stderr.strip().splitlines()[0])
+def test_welford_cov_kernel_sources_are_data_race_free_under_thread_sanitizer():
+    r = E.sanitized("dense_adapt", "thread")
     assert r.returncode == 0 and "WARNING: ThreadSanitizer" not in r.stderr, r.stdout + r.stderr[-3000:]
     assert r.stdout.count("rc 0") == 4, r.stdout

@@ -9,54 +9,25 @@ tests/test_dense_user_adapt.py."""
 import concurrent.futures as cf
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import ahmc_b200 as A
 from oracle import oracle_c as oc
+from tests import emu as E
 from tests import philox_ref as R
+from tests.emu import P, EmuDenseUserAdapt
 from tests.helpers import rel_err
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU = os.path.join(ROOT, "tests", "simt_emu")
-CSRC = os.path.join(ROOT, "advancedhmc.jl_b200", "csrc")
-_vp = C.c_void_p
-P = lambda a: None if a is None else a.ctypes.data_as(_vp)
 WELFORD_COV = 3
 UK_NUTS_ADAPT, UK_HMC_ADAPT = 5, 6
 
 
-class EmuDenseUserAdapt(C.Structure):
-    _fields_ = [("hmc", C.c_int32), ("D", C.c_int32), ("N", C.c_int64), ("params", _vp), ("Minv0", _vp), ("cholU0", _vp),
-                ("metric_stride", C.c_int64), ("eps0", C.c_double), ("max_depth", C.c_int32), ("n_steps", C.c_int32),
-                ("seed", C.c_uint64), ("T", C.c_int32), ("n_adapts", C.c_int32), ("init_buffer", C.c_int32),
-                ("term_buffer", C.c_int32), ("window_size", C.c_int32), ("adapt_metric", C.c_int32), ("n_min", C.c_int32),
-                ("th_in", _vp), ("g_in", _vp), ("lp_in", _vp), ("th_out", _vp), ("r_out", _vp), ("g_out", _vp), ("lp_out", _vp),
-                ("lk_out", _vp), ("draws", _vp), ("acc", _vp), ("eps_trace", _vp), ("n_steps_out", _vp), ("tree_depth", _vp),
-                ("is_accept", _vp), ("numerical", _vp), ("eps_rw", _vp), ("minv_rw", _vp), ("cholu_rw", _vp)]
-
-
-def _gxx(out, form, *extra):
-    return ["g++", *extra, "-std=c++20", "-pthread", "-ffp-contract=off", "-w", *(["-DDENSE_USER_GROUP"] if form == "group" else []),
-            "-I", os.path.join(EMU, "include"), "-I", CSRC, "-I", os.path.join(ROOT, "include"), os.path.join(EMU, "simt_emu.cpp"),
-            os.path.join(EMU, "dense_user_adapt_emu.cpp"), "-o", str(out)]
-
-
 @pytest.fixture(scope="module")
-def emus(tmp_path_factory):
-    """the harness in the group form and the one-lane form, compiled once each (in parallel)"""
-    tmp = tmp_path_factory.mktemp("simt_dense_user_adapt")
-
-    def build(form):
-        out = tmp / f"libdense_user_adapt_{form}.so"
-        pr = subprocess.run(_gxx(out, form, "-O1", "-shared", "-fPIC"), capture_output=True, text=True)
-        assert pr.returncode == 0, pr.stderr[-2000:]
-        return form, C.CDLL(str(out))
-
-    with cf.ThreadPoolExecutor(max_workers=2) as ex:
-        return dict(ex.map(build, ("group", "one_lane")))
+def emus():
+    """the harness in the group form and the one-lane form"""
+    return dict(zip(("group", "one_lane"), E.harnesses(("dense_user_adapt", "DENSE_USER_GROUP"), "dense_user_adapt")))
 
 
 def _spd(rng, D, lo=-0.3, hi=0.3):
@@ -178,16 +149,8 @@ def test_welford_cov_user_kernels_under_emulation_equal_the_oracle_iteration_by_
 
 
 @pytest.mark.parametrize("form", ["group", "one_lane"])
-def test_welford_cov_user_kernels_are_data_race_free_under_thread_sanitizer(tmp_path, form):
-    out = tmp_path / f"race_dense_user_adapt_{form}"
-    pr = subprocess.run(_gxx(out, form, "-DDENSE_USER_ADAPT_RACE", "-O1", "-g", "-fsanitize=thread", "-x", "c++"),
-                        capture_output=True, text=True)
-    if pr.returncode != 0 and "tsan" in pr.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available to g++ here")
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    r = subprocess.run([str(out)], capture_output=True, text=True, timeout=900)
-    if "FATAL: ThreadSanitizer" in r.stderr:
-        pytest.skip("ThreadSanitizer cannot run in this environment: " + r.stderr.strip().splitlines()[0])
+def test_welford_cov_user_kernels_are_data_race_free_under_thread_sanitizer(form):
+    r = E.sanitized("dense_user_adapt", "thread", *(["DENSE_USER_GROUP"] if form == "group" else []))
     assert r.returncode == 0 and "WARNING: ThreadSanitizer" not in r.stderr, r.stdout + r.stderr[-3000:]
     assert r.stdout.count("rc 0") == 4, r.stdout
 
@@ -230,25 +193,11 @@ __device__ double ahmc_user_logp_grad_group(const double* th, double* g, int D, 
 '''
 
 
-def _lib_or_skip():
-    lib = A._lib.load()
-    log = C.create_string_buffer(4096)
-    if lib.ahmc_user_source_check(ONE_LANE.encode(), 0, 0, 3, log, 4096) == A._lib.ERR_UNSUPPORTED:
-        pytest.skip("libnvrtc not available here: " + log.value.decode())
-    return lib
-
-
-def _check(lib, src, kernel, metric, D):
-    log = C.create_string_buffer(8192)
-    rc = lib.ahmc_user_source_check(src.encode(), kernel, metric, D, log, 8192)
-    return rc, log.value.decode()
-
-
 def test_adaptive_kernels_with_the_dense_kind_compile_for_every_source_contract_and_the_glm_source():
     """kernels 5 and 6 (adaptive NUTS, adaptive static HMC) with metric_kind = Dense compile the WelfordCov form on the
     per-chain Dense kind, for the one-lane, coordinate-wise and group forms at D = 6 (G = 8, several chains per warp) and
     D = 40 (G = 32), and for the Bernoulli-logit source a GLMTarget generates"""
-    lib = _lib_or_skip()
+    lib = E.nvrtc_lib_or_skip()
     rng = np.random.default_rng(3)
     X = rng.normal(size=(50, 40))
     glm = A.GLMTarget(X, (rng.uniform(size=50) < 0.5).astype(float), "bernoulli_logit", prior_prec=1.0).source()
@@ -256,13 +205,13 @@ def test_adaptive_kernels_with_the_dense_kind_compile_for_every_source_contract_
             for kernel in (UK_NUTS_ADAPT, UK_HMC_ADAPT)]
     jobs += [(glm, kernel, A._lib.METRIC_DENSE, 40) for kernel in (UK_NUTS_ADAPT, UK_HMC_ADAPT)]
     with cf.ThreadPoolExecutor(max_workers=os.cpu_count() or 4) as ex:
-        results = list(ex.map(lambda j: _check(lib, *j), jobs))
+        results = list(ex.map(lambda j: E.source_check(lib, *j), jobs))
     for (src, kernel, metric, D), (rc, log) in zip(jobs, results):
         assert rc == 0, (kernel, metric, D, src[:40], log[-2000:])
 
 
 def test_a_broken_source_checked_for_the_dense_warm_up_comes_back_with_its_log():
-    lib = _lib_or_skip()
+    lib = E.nvrtc_lib_or_skip()
     for kernel in (UK_NUTS_ADAPT, UK_HMC_ADAPT):
-        rc, log = _check(lib, GROUPWISE.replace("return grp.lane == 0", "return nope == 0"), kernel, A._lib.METRIC_DENSE, 6)
+        rc, log = E.source_check(lib, GROUPWISE.replace("return grp.lane == 0", "return nope == 0"), kernel, A._lib.METRIC_DENSE, 6)
         assert rc == A._lib.ERR_INVALID and "nope" in log and "undefined" in log, log

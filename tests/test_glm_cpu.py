@@ -3,42 +3,20 @@ float64 numpy statement of the target (tests/glm_ref.py), the stable link-functi
 the generated group-form source through the compile-only check."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
-import ahmc_b200 as A
+from tests import emu as E
 from tests import glm_ref as R
+from tests.emu import P, EmuGlm
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_vp = C.c_void_p
 FAM = {"bernoulli_logit": 0, "poisson_log": 1}
 
 
-class EmuGlm(C.Structure):
-    _fields_ = [("family", C.c_int32), ("D", C.c_int32), ("n", C.c_int32), ("N", C.c_int64), ("X", _vp), ("y", _vp), ("prec", _vp),
-                ("c0", C.c_double), ("Minv", _vp), ("chain_stride", C.c_int64), ("eps", C.c_double), ("eps_chain", _vp),
-                ("n_steps", C.c_int32), ("fwd", C.c_int32), ("th_in", _vp), ("r_in", _vp), ("g_in", _vp), ("th_out", _vp),
-                ("r_out", _vp), ("g_out", _vp), ("dr_out", _vp), ("lp_out", _vp), ("lk_out", _vp), ("status", _vp),
-                ("steps_done", _vp), ("nc_out", C.c_int32), ("stages_out", C.c_int32)]
-
-
-def P(a):
-    return None if a is None else a.ctypes.data_as(_vp)
-
-
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    tmp = tmp_path_factory.mktemp("simt_glm")
-    d = os.path.join(ROOT, "tests", "simt_emu")
-    out = tmp / "libglm_emu.so"
-    cmd = ["g++", "-O1", "-std=c++20", "-shared", "-fPIC", "-pthread", "-ffp-contract=off", "-x", "c++",
-           "-I", os.path.join(d, "include"), "-I", os.path.join(ROOT, "advancedhmc.jl_b200", "csrc"),
-           "-I", os.path.join(ROOT, "include"), os.path.join(d, "simt_emu.cpp"), os.path.join(d, "glm_emu.cpp"), "-o", str(out)]
-    pr = subprocess.run(cmd, capture_output=True, text=True)
-    assert pr.returncode == 0, pr.stderr[-3000:]
-    return C.CDLL(str(out))
+def emu():
+    return E.harness("glm")
 
 
 def run_emu(lib, family, X, y, prec, c0, Minv, eps, n_steps, th, r, g, in_place=False):
@@ -139,7 +117,7 @@ def test_stable_link_branches_match_50_digit_values():
     softplus / sigmoid overflows; Poisson at eta = 750 is non-finite."""
     import json
 
-    gold = json.load(open(os.path.join(ROOT, "tests", "golden", "glm_mp50.json")))
+    gold = json.load(open(os.path.join(E.ROOT, "tests", "golden", "glm_mp50.json")))
     for case in gold["cases"]:
         X, y, th = np.array(case["X"]), np.array(case["y"]), np.array(case["theta"])[None, :]
         prec = np.array(case["prec"])
@@ -155,7 +133,7 @@ def test_stable_link_branches_match_50_digit_values():
 def test_emulated_kernel_matches_50_digit_values(emu):
     import json
 
-    gold = json.load(open(os.path.join(ROOT, "tests", "golden", "glm_mp50.json")))
+    gold = json.load(open(os.path.join(E.ROOT, "tests", "golden", "glm_mp50.json")))
     for case in gold["cases"]:
         X, y, th = np.array(case["X"]), np.array(case["y"]), np.array(case["theta"])[None, :]
         c0 = 0.0 - (0 if case["family"] == "bernoulli_logit" else R.gammaln(y + 1).sum())
@@ -182,15 +160,12 @@ def test_tile_shapes_fit_shared_memory(emu):
 @pytest.mark.parametrize("D", [3, 25, 100, 300])
 def test_generated_group_source_compiles(family, D):
     """the source a GLM target runs as on the run-time compiled kernels passes the compile-only check (needs NVRTC, no GPU)"""
-    lib = A._lib.load()
-    log = C.create_string_buffer(4096)
-    probe = "__device__ double ahmc_user_logp_grad(const double* t, double* g, int D, const double* p) { return 0.0; }"
-    if lib.ahmc_user_source_check(probe.encode(), 1, 1, 4, log, 4096) == A._lib.ERR_UNSUPPORTED:
-        pytest.skip("NVRTC is not available: " + log.value.decode())
+    lib = E.nvrtc_lib_or_skip()
     n = lib.ahmc_glm_source(FAM[family], D, 1000, None, 0)
     buf = C.create_string_buffer(n + 1)
     assert lib.ahmc_glm_source(FAM[family], D, 1000, buf, n + 1) == n
     src = buf.value
     assert b"AHMC_USER_GROUPWISE" in src and f"GLM_D {D}".encode() in src
     for kernel, metric in ((1, 0), (2, 1), (3, 2)):
-        assert lib.ahmc_user_source_check(src, kernel, metric, D, log, 4096) == 0, log.value.decode()
+        rc, log = E.source_check(lib, src, kernel, metric, D)
+        assert rc == 0, log

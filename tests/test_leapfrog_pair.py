@@ -3,27 +3,20 @@ forms (one set shared by the pair; per-chain eps and M^-1), ragged N, and pairs 
 and is re-run alone by the exact path.  The CPU tests run the kernel source under the SIMT emulator at D = 64
 (tests/simt_emu/pair_emu.cpp), against the oracle and under ThreadSanitizer; the GPU test runs the library at D = 128."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import oracle_c as oc
+from tests import emu as E
+from tests.emu import P, EmuLf
 from tests.helpers import rel_err
-from tests.test_simt_emulation import KINDS, MKINDS, EmuLf, P, _lf_system
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU = os.path.join(ROOT, "tests", "simt_emu")
-INCLUDES = ["-I", os.path.join(EMU, "include"), "-I", os.path.join(ROOT, "advancedhmc.jl_b200", "csrc"), "-I", os.path.join(ROOT, "include")]
+from tests.test_simt_emulation import KINDS, MKINDS, _lf_system
 
 
 @pytest.fixture(scope="module")
-def emu_pair(tmp_path_factory):
-    out = tmp_path_factory.mktemp("simt_pair") / "libpair_emu.so"
-    subprocess.run(["g++", "-O1", "-std=c++20", "-shared", "-fPIC", "-pthread", "-ffp-contract=off", "-x", "c++", *INCLUDES,
-                    os.path.join(EMU, "simt_emu.cpp"), os.path.join(EMU, "pair_emu.cpp"), "-o", str(out)], check=True)
-    return C.CDLL(str(out))
+def emu_pair():
+    return E.harness("pair")
 
 
 @pytest.mark.parametrize("per_chain_eps", [False, True], ids=["shared-coef", "chain-eps"])
@@ -58,19 +51,10 @@ def test_pair_kernel_under_emulation_matches_oracle(emu_pair, per_chain_eps, wit
     assert lp_o[5] == -np.inf
 
 
-def test_pair_kernel_source_is_data_race_free_under_thread_sanitizer(tmp_path):
+def test_pair_kernel_source_is_data_race_free_under_thread_sanitizer():
     """Every CUDA thread is a host thread whose only synchronisation is what the kernel asks for: a missing __syncwarp
     between A's and B's use of the warp (votes, reductions, the exact path's shared-memory slab) is a reported race."""
-    exe = tmp_path / "race_pair"
-    b = subprocess.run(["g++", "-DPAIR_RACE_MAIN", "-w", "-O1", "-g", "-std=c++20", "-pthread", "-fsanitize=thread", "-ffp-contract=off",
-                        "-x", "c++", *INCLUDES, os.path.join(EMU, "simt_emu.cpp"), os.path.join(EMU, "pair_emu.cpp"), "-o", str(exe)],
-                       capture_output=True, text=True)
-    if b.returncode != 0 and ("tsan" in b.stderr.lower() or "sanitize" in b.stderr.lower()):
-        pytest.skip("ThreadSanitizer runtime not available to g++ here")
-    assert b.returncode == 0, b.stderr[-2000:]
-    r = subprocess.run([str(exe)], capture_output=True, text=True, timeout=600)
-    if "FATAL: ThreadSanitizer" in r.stderr:
-        pytest.skip("ThreadSanitizer cannot run in this environment: " + r.stderr.strip().splitlines()[0])
+    r = E.sanitized("pair", "thread", timeout=600)
     assert r.stderr.count("WARNING: ThreadSanitizer: data race") == 0 and r.returncode == 0, r.stderr[-3000:] + r.stdout[-500:]
     assert r.stdout.count("rc 0 finished 11 of 11") == 2
 

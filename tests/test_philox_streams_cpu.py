@@ -4,17 +4,13 @@ rule of every register layout, and the device source itself -- Philox::gen, phil
 big_normals and the exponential / direction-bit draws -- run on the CPU (tests/simt_emu/philox_emu.cpp) against the
 restatement.  The GPU side is tests/test_philox_streams.py."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from tests import emu as E
 from tests import philox_ref as P
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU = os.path.join(ROOT, "tests", "simt_emu")
-CSRC = os.path.join(ROOT, "advancedhmc.jl_b200", "csrc")
 SEEDS = [0, 1, 2026, 2**32 + 17, 0xDEADBEEFCAFEF00D]  # seeds >= 2^32: key word k1 != 0
 OFFSETS = [0, 1, 2**35 + 3, 2**36 - 1]
 
@@ -27,14 +23,8 @@ KAT = [
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    out = tmp_path_factory.mktemp("simt_philox") / "libphilox_emu.so"
-    cmd = ["g++", "-O1", "-shared", "-fPIC", "-std=c++20", "-pthread", "-ffp-contract=off", "-w", "-I", os.path.join(EMU, "include"),
-           "-I", CSRC, "-I", os.path.join(ROOT, "include"), os.path.join(EMU, "simt_emu.cpp"), os.path.join(EMU, "philox_emu.cpp"),
-           "-o", str(out)]
-    pr = subprocess.run(cmd, capture_output=True, text=True)
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    lib = C.CDLL(str(out))
+def emu():
+    lib = E.harness("philox")
     lib.emu_philox_u01.restype = C.c_double
     lib.emu_philox_u01.argtypes = [C.c_uint32, C.c_uint32]
     for f in (lib.emu_philox_normals, lib.emu_big_normals):

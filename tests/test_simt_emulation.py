@@ -3,51 +3,25 @@ on the CPU by a small SIMT emulator (tests/simt_emu/: one host thread per CUDA t
 a barrier in every shuffle / vote) and compared with the recursive C oracle on shared random tapes.  This checks the
 kernel's actual code -- control flow, workspace addressing, warp-uniform predicates, every template family -- without a
 GPU; the GPU parity tests (-m gpu) remain the authority for the compiled binary."""
+import concurrent.futures as cf
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import oracle_c as oc
+from tests import emu as E
+from tests.emu import P, EmuDense, EmuLf, EmuMn, EmuNuts
 from tests.helpers import rel_err
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_vp = C.c_void_p
-
-
-class EmuNuts(C.Structure):
-    _fields_ = [("model_kind", C.c_int32), ("metric_kind", C.c_int32), ("D", C.c_int32), ("N", C.c_int64), ("p0", _vp), ("p1", _vp),
-                ("c0", C.c_double), ("Minv", _vp), ("minv_stride", C.c_int64), ("cholU", _vp), ("eps", C.c_double),
-                ("eps_chain", _vp), ("max_depth", C.c_int32), ("delta_max", C.c_double), ("sampler", C.c_int32),
-                ("criterion", C.c_int32), ("seed", C.c_uint64), ("offset", C.c_uint64), ("normal_tape", _vp), ("exp_tape", _vp),
-                ("exp_stride", C.c_int64), ("dir_tape", _vp), ("dir_stride", C.c_int64), ("partial_alpha", C.c_double),
-                ("refresh", C.c_int32), ("th_in", _vp), ("r_in", _vp), ("g_in", _vp), ("lp_in", _vp), ("th_out", _vp),
-                ("r_out", _vp), ("g_out", _vp), ("lp_out", _vp), ("lk_out", _vp), ("n_steps", _vp), ("tree_depth", _vp),
-                ("numerical", _vp), ("acc", _vp), ("dH", _vp), ("dHmax", _vp), ("n_transitions", C.c_int32), ("draws", _vp),
-                ("adapt", C.c_int32), ("n_adapts", C.c_int32), ("init_buffer", C.c_int32), ("term_buffer", C.c_int32),
-                ("window_size", C.c_int32), ("delta", C.c_double), ("gamma", C.c_double), ("t0", C.c_double), ("kappa", C.c_double),
-                ("adapt_metric", C.c_int32), ("n_min", C.c_int32), ("eps_rw", _vp), ("minv_rw", _vp), ("eps_trace", _vp),
-                ("temper_alpha", C.c_double), ("coop_padded", C.c_int32)]
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    """the NUTS harness (kernel source + emulator), compiled once per test module"""
-    tmp = tmp_path_factory.mktemp("simt_nuts")
-    d = os.path.join(ROOT, "tests", "simt_emu")
-    out = tmp / "libnuts_emu.so"
-    cmd = ["g++", "-O1", "-std=c++20", "-shared", "-fPIC", "-pthread", "-ffp-contract=off", "-I", os.path.join(d, "include"),
-           "-I", os.path.join(ROOT, "advancedhmc.jl_b200", "csrc"), "-I", os.path.join(ROOT, "include"),
-           os.path.join(d, "simt_emu.cpp"), os.path.join(d, "nuts_emu.cpp"), "-o", str(out)]
-    pr = subprocess.run(cmd, capture_output=True, text=True)
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    return C.CDLL(str(out))
+def emu():
+    """the NUTS harness (kernel source + emulator)"""
+    return E.harness("nuts")
 
 
-
-P = lambda a: None if a is None else a.ctypes.data_as(_vp)
 KINDS = dict(std_normal=oc.STD_NORMAL, diag_gauss=oc.DIAG_GAUSS, dense_gauss=oc.DENSE_GAUSS, funnel=oc.FUNNEL)
 MKINDS = dict(unit=oc.UNIT, diag=oc.DIAG, dense=oc.DENSE)
 
@@ -246,25 +220,9 @@ def test_in_launch_adaptation_under_emulation_equals_oracle_adaptors(emu):
 
 
 # ------------------------------------------------------------------------------------------------ K1 / K2 under emulation
-class EmuLf(C.Structure):
-    _fields_ = [("model_kind", C.c_int32), ("metric_kind", C.c_int32), ("D", C.c_int32), ("N", C.c_int64), ("p0", _vp), ("p1", _vp),
-                ("c0", C.c_double), ("Minv", _vp), ("minv_stride", C.c_int64), ("cholU", _vp), ("eps", C.c_double),
-                ("eps_chain", _vp), ("n_steps", C.c_int32), ("fwd", C.c_int32), ("temper_alpha", C.c_double), ("th_in", _vp),
-                ("r_in", _vp), ("g_in", _vp), ("lp_in", _vp), ("th_out", _vp), ("r_out", _vp), ("g_out", _vp), ("lp_out", _vp),
-                ("lk_out", _vp), ("dr_out", _vp), ("status", _vp), ("steps_done", _vp), ("flags", C.c_uint32), ("hmc", C.c_int32),
-                ("refresh", C.c_int32), ("n_transitions", C.c_int32), ("seed", C.c_uint64), ("offset", C.c_uint64),
-                ("normal_tape", _vp), ("exp_tape", _vp), ("is_accept", _vp), ("acc", _vp), ("dH", _vp), ("draws", _vp)]
-
-
 @pytest.fixture(scope="module")
-def emu_lf(tmp_path_factory):
-    out = tmp_path_factory.mktemp("simt_lf") / "liblf_emu.so"
-    d = os.path.join(ROOT, "tests", "simt_emu")
-    subprocess.run(["g++", "-O1", "-std=c++20", "-shared", "-fPIC", "-pthread", "-ffp-contract=off", "-x", "c++",
-                    "-I", os.path.join(d, "include"), "-I", os.path.join(ROOT, "advancedhmc.jl_b200", "csrc"),
-                    "-I", os.path.join(ROOT, "include"), os.path.join(d, "simt_emu.cpp"), os.path.join(d, "lf_emu.cpp"),
-                    "-o", str(out)], check=True)
-    return C.CDLL(str(out))
+def emu_lf():
+    return E.harness("lf")
 
 
 def _lf_system(kind, mkind, D, rng):
@@ -394,22 +352,9 @@ def test_kernel_source_emulated_randomised_configurations(emu):
 
 
 # ------------------------------------------------------------------------------------------------ MultinomialTS static kernel
-class EmuMn(C.Structure):
-    _fields_ = [("model_kind", C.c_int32), ("metric_kind", C.c_int32), ("D", C.c_int32), ("N", C.c_int64), ("p0", _vp), ("p1", _vp),
-                ("Minv", _vp), ("cholU", _vp), ("eps", C.c_double), ("n_steps", C.c_int32), ("n_fwd", C.c_int32),
-                ("normal_tape", _vp), ("unif_tape", _vp), ("th_in", _vp), ("g_in", _vp), ("lp_in", _vp), ("th_out", _vp),
-                ("r_out", _vp), ("g_out", _vp), ("lp_out", _vp), ("lk_out", _vp), ("acc", _vp), ("index", _vp), ("temper_alpha", C.c_double)]
-
-
 @pytest.fixture(scope="module")
-def emu_mn(tmp_path_factory):
-    out = tmp_path_factory.mktemp("simt_mn") / "libmn_emu.so"
-    d = os.path.join(ROOT, "tests", "simt_emu")
-    subprocess.run(["g++", "-O1", "-std=c++20", "-shared", "-fPIC", "-pthread", "-ffp-contract=off", "-x", "c++",
-                    "-I", os.path.join(d, "include"), "-I", os.path.join(ROOT, "advancedhmc.jl_b200", "csrc"),
-                    "-I", os.path.join(ROOT, "include"), os.path.join(d, "simt_emu.cpp"), os.path.join(d, "mn_emu.cpp"),
-                    "-o", str(out)], check=True)
-    return C.CDLL(str(out))
+def emu_mn():
+    return E.harness("mn")
 
 
 def test_multinomial_static_kernel_source_under_emulation_matches_mp50_fixtures(emu_mn):
@@ -487,16 +432,10 @@ def test_multinomial_static_with_tempered_leapfrog_under_emulation_matches_oracl
     assert not np.allclose(su.acceptance_rate, so.acceptance_rate, rtol=1e-6)
 
 
-def test_adaptor_statistics_kernel_sources_under_emulation(tmp_path):
+def test_adaptor_statistics_kernel_sources_under_emulation():
     """K5 (`adapt_kernel`: per-block partials, last-block reduction through a device counter) and K5b (`adapt_cov_kernel`:
     tiled second moment) executed by the emulator (block barriers, static shared variables) vs numpy."""
-    out = tmp_path / "libadapt_emu.so"
-    d = os.path.join(ROOT, "tests", "simt_emu")
-    subprocess.run(["g++", "-O1", "-std=c++20", "-shared", "-fPIC", "-pthread", "-ffp-contract=off", "-x", "c++",
-                    "-I", os.path.join(d, "include"), "-I", os.path.join(ROOT, "advancedhmc.jl_b200", "csrc"),
-                    "-I", os.path.join(ROOT, "include"), os.path.join(d, "simt_emu.cpp"), os.path.join(d, "adapt_emu.cpp"),
-                    "-o", str(out)], check=True)
-    lib = C.CDLL(str(out))
+    lib = E.harness("adapt")
     rng = np.random.default_rng(8)
     for D, N in ((7, 33), (40, 13), (33, 3)):
         Lm = rng.normal(size=(D, D)) / np.sqrt(D)
@@ -513,23 +452,17 @@ def test_adaptor_statistics_kernel_sources_under_emulation(tmp_path):
 
 
 @pytest.mark.parametrize("R,adapt_metric", [(1, 1), (2, 1), (5, 1), (3, 0)])
-def test_pooled_adaptor_kernel_source_under_emulation_equals_host_adaptors(tmp_path, R, adapt_metric):
+def test_pooled_adaptor_kernel_source_under_emulation_equals_host_adaptors(R, adapt_metric):
     """The device-side exchange's arithmetic (`pooled_update_kernel`, ahmc_pooled.cu: rank-ordered Chan merge of R per-rank
     records, NesterovDualAveraging, WelfordVar, Stan windows, reset / finalize) executed by the CPU emulator on the records R
     ranks would all-gather, against the host-side pooled adaptors of adaptation.py fed with the merged record -- the N > 1
     path of the exchange without a GPU or NCCL (the GPU suite repeats it over a real 2-rank communicator)."""
     from ahmc_b200 import adaptation as ad
 
-    out = tmp_path / "libpooled_emu.so"
-    d = os.path.join(ROOT, "tests", "simt_emu")
-    subprocess.run(["g++", "-O1", "-std=c++20", "-shared", "-fPIC", "-pthread", "-ffp-contract=off", "-x", "c++",
-                    "-I", os.path.join(d, "include"), "-I", os.path.join(ROOT, "advancedhmc.jl_b200", "csrc"),
-                    "-I", os.path.join(ROOT, "include"), os.path.join(d, "simt_emu.cpp"), os.path.join(d, "pooled_emu.cpp"),
-                    "-o", str(out)], check=True)
-    lib = C.CDLL(str(out))
+    lib = E.harness("pooled")
     lib.emu_pooled_create.restype = C.c_void_p
     lib.emu_pooled_create.argtypes = [C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int]
-    lib.emu_pooled_update.argtypes = [C.c_void_p, _vp, C.c_int, _vp, _vp, _vp]
+    lib.emu_pooled_update.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.emu_pooled_destroy.argtypes = [C.c_void_p]
     D, n_adapts, windows = 13, 40, (5, 4, 6)
     rng = np.random.default_rng(17 + R)
@@ -609,25 +542,9 @@ def test_trajectory_kernel_emulated_nonfinite_freeze_tempering_and_fast_path_fal
 
 
 # ---------------------------------------------------------------------------------------------------------------- K4
-class EmuDense(C.Structure):
-    _fields_ = [("D", C.c_int32), ("N", C.c_int64), ("P", _vp), ("w", _vp), ("mu", _vp), ("c0", C.c_double), ("Minv", _vp),
-                ("Mdiag", _vp), ("eps", C.c_double), ("eps_chain", _vp), ("n_steps", C.c_int32), ("fwd", C.c_int32),
-                ("th_in", _vp), ("r_in", _vp), ("g_in", _vp), ("th_out", _vp), ("r_out", _vp), ("g_out", _vp), ("dr_out", _vp),
-                ("lp_out", _vp), ("lk_out", _vp), ("status", _vp), ("steps_done", _vp), ("need_exact", _vp),
-                ("wide_tile", C.c_int32), ("norms_out", C.c_double * 2)]
-
-
 @pytest.fixture(scope="module")
-def emu_dense(tmp_path_factory):
-    tmp = tmp_path_factory.mktemp("simt_dense")
-    d = os.path.join(ROOT, "tests", "simt_emu")
-    out = tmp / "libdense_emu.so"
-    cmd = ["g++", "-O1", "-std=c++20", "-shared", "-fPIC", "-pthread", "-ffp-contract=off", "-x", "c++",
-           "-I", os.path.join(d, "include"), "-I", os.path.join(ROOT, "advancedhmc.jl_b200", "csrc"),
-           "-I", os.path.join(ROOT, "include"), os.path.join(d, "simt_emu.cpp"), os.path.join(d, "dense_emu.cpp"), "-o", str(out)]
-    pr = subprocess.run(cmd, capture_output=True, text=True)
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    lib = C.CDLL(str(out))
+def emu_dense():
+    lib = E.harness("dense")
     assert lib.emu_dense_stages() == 3
     return lib
 
@@ -649,8 +566,7 @@ def _dense_run(lib, kind, mkind, D, N, eps, n, fwd, seed, per_chain_eps=True, wi
     w = dp1 if kind == "diag_gauss" else None
     Mm = np.asfortranarray(Minv) if mkind == "dense" else None
     Md = Minv if mkind == "diag" else None
-    q = EmuDense(D=D, N=N, P=None if Pm is None else Pm.ctypes.data_as(_vp), w=P(w), mu=P(p0), c0=0.0,
-                 Minv=None if Mm is None else Mm.ctypes.data_as(_vp), Mdiag=P(Md), eps=eps, eps_chain=P(eps_chain), n_steps=n,
+    q = EmuDense(D=D, N=N, P=P(Pm), w=P(w), mu=P(p0), c0=0.0, Minv=P(Mm), Mdiag=P(Md), eps=eps, eps_chain=P(eps_chain), n_steps=n,
                  fwd=fwd, th_in=P(th), r_in=P(r), g_in=P(g_in), th_out=P(o["th"]), r_out=P(o["r"]), g_out=P(o["g"]),
                  dr_out=P(o["dr"]), lp_out=P(lp_o), lk_out=P(lk_o), status=P(status), steps_done=P(done), need_exact=P(need),
                  wide_tile=wide)
@@ -691,52 +607,29 @@ def test_dense_tile_kernel_emulated_hands_a_suspect_tile_to_the_exact_kernel(emu
 
 
 # ------------------------------------------------------------------------------- data-race check of the kernel sources
-_RACE_BUILDS = {  # name -> compile-time definitions for tests/simt_emu/race_main.cpp
-    "nuts": ["-DRACE_NUTS"],
-    "lf": ["-DRACE_LF"],
-    "multinomial": ["-DRACE_MN"],
-    "adapt": ["-DRACE_ADAPT"],
-    "dense": ["-DRACE_DENSE"],
-    "dense-mutant": ["-DRACE_DENSE"]}  # a copy of ahmc_dense.cu with one barrier removed: the detector must fire
+_RACE_HARNESS = {"nuts": "nuts", "lf": "lf", "multinomial": "mn", "adapt": "adapt", "dense": "dense",
+                 "dense-mutant": "dense"}  # with a copy of ahmc_dense.cu with one barrier removed: the detector must fire
 
 
 @pytest.fixture(scope="module")
-def _race_bins(tmp_path_factory):
-    tmp = tmp_path_factory.mktemp("simt_race")
-    d = os.path.join(ROOT, "tests", "simt_emu")
-    csrc = os.path.join(ROOT, "advancedhmc.jl_b200", "csrc")
-    src = open(os.path.join(csrc, "ahmc_dense.cu")).read()
+def _race_runs(tmp_path_factory):
+    """each program's outcome (the run, or the skip), all built and run at once"""
+    mut = tmp_path_factory.mktemp("mutant")
+    src = open(os.path.join(E.CSRC, "ahmc_dense.cu")).read()
     barrier = "= v[rb][cb][j];\n    __syncthreads();"  # tile_to_smem: publish the staged vectors to the other warps
     assert src.count(barrier) == 1
-    mut = tmp / "mutant"
-    mut.mkdir()
     (mut / "ahmc_dense.cu").write_text(src.replace(barrier, "= v[rb][cb][j];"))
-    procs = {}
-    for name, defs in _RACE_BUILDS.items():
-        out = tmp / f"race_{name}"
-        inc = ["-I", str(mut)] if name == "dense-mutant" else []
-        cmd = ["g++", *defs, "-w", "-O1", "-g", "-std=c++20", "-pthread", "-fsanitize=thread", "-ffp-contract=off", "-x", "c++", *inc,
-               "-I", os.path.join(d, "include"), "-I", csrc, "-I", os.path.join(ROOT, "include"), os.path.join(d, "simt_emu.cpp"),
-               os.path.join(d, "race_main.cpp"), "-o", str(out)]
-        procs[name] = (subprocess.Popen(cmd, stderr=subprocess.PIPE, text=True), out)
-    bins = {}
-    for name, (pr, out) in procs.items():
-        _, err = pr.communicate()
-        if pr.returncode != 0 and ("tsan" in err.lower() or "sanitize" in err.lower()):
-            pytest.skip("ThreadSanitizer runtime not available to g++ here")
-        assert pr.returncode == 0, err[-2000:]
-        bins[name] = str(out)
-    return bins
+    with cf.ThreadPoolExecutor(max_workers=len(_RACE_HARNESS)) as ex:
+        return {name: ex.submit(E.sanitized, h, "thread", include_first=str(mut) if name == "dense-mutant" else None, timeout=600)
+                for name, h in _RACE_HARNESS.items()}
 
 
-@pytest.mark.parametrize("name", list(_RACE_BUILDS))
-def test_kernel_sources_are_data_race_free_under_thread_sanitizer(_race_bins, name):
+@pytest.mark.parametrize("name", list(_RACE_HARNESS))
+def test_kernel_sources_are_data_race_free_under_thread_sanitizer(_race_runs, name):
     """Every CUDA thread is a host thread whose only synchronisation is what the kernel asks for, so ThreadSanitizer sees a
     missing __syncwarp / __syncthreads / mbarrier wait as a data race: the shipped NUTS, trajectory / HMC, MultinomialTS, adaptor-statistics
     and dense-tile sources must be clean, and a copy of the dense kernel with one barrier removed must be reported."""
-    r = subprocess.run([_race_bins[name]], capture_output=True, text=True, timeout=600)
-    if "FATAL: ThreadSanitizer" in r.stderr:
-        pytest.skip("ThreadSanitizer cannot run in this environment: " + r.stderr.strip().splitlines()[0])
+    r = _race_runs[name].result()
     races = r.stderr.count("WARNING: ThreadSanitizer: data race")
     if name == "dense-mutant":
         assert races > 0 and "dense_traj_kernel" in r.stderr

@@ -11,7 +11,6 @@ warps.  Each emulated run happens in a forked child, so a contract violation (th
 it) fails the one test instead of ending the session."""
 import ctypes as C
 import os
-import subprocess
 import sys
 import traceback
 
@@ -19,35 +18,20 @@ import numpy as np
 import pytest
 
 from oracle import oracle_c as oc
+from tests import emu as E
 from tests import glm_ref as R
+from tests.emu import P, EmuNuts
 from tests.helpers import rel_err
 from tests.test_glm_cpu import _setup as _glm_setup, assert_z, close, run_emu as _glm_run
-from tests.test_simt_emulation import EmuNuts, _case as _nuts_case, _dense_run
+from tests.test_simt_emulation import _case as _nuts_case, _dense_run
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU = os.path.join(ROOT, "tests", "simt_emu")
-_vp = C.c_void_p
 POISON_NAN, POISON_HUGE = 0, 1
 
 
-def _gxx(src, out, *extra):
-    return ["g++", *extra, "-std=c++20", "-pthread", "-ffp-contract=off", "-w", "-x", "c++", "-I", os.path.join(EMU, "include"),
-            "-I", os.path.join(ROOT, "advancedhmc.jl_b200", "csrc"), "-I", os.path.join(ROOT, "include"),
-            os.path.join(EMU, "simt_emu.cpp"), os.path.join(EMU, src), "-o", str(out)]
-
-
 @pytest.fixture(scope="module")
-def libs(tmp_path_factory):
-    """the K4, K6 and NUTS harnesses on the strict emulator, compiled in parallel"""
-    tmp = tmp_path_factory.mktemp("tensor_pipe_cpu")
-    procs = {k: (subprocess.Popen(_gxx(f"{k}_emu.cpp", tmp / f"lib{k}.so", "-O1", "-shared", "-fPIC"), stderr=subprocess.PIPE,
-                                  text=True), tmp / f"lib{k}.so") for k in ("dense", "glm", "nuts")}
-    out = {}
-    for k, (pr, so) in procs.items():
-        _, err = pr.communicate()
-        assert pr.returncode == 0, err[-3000:]
-        out[k] = C.CDLL(str(so))
-    return out
+def libs():
+    """the K4, K6 and NUTS harnesses on the strict emulator"""
+    return dict(zip(("dense", "glm", "nuts"), E.harnesses("dense", "glm", "nuts")))
 
 
 def isolated(lib, poison, fn, *args, **kw):
@@ -240,7 +224,6 @@ def _coop_multi(lib, D, N, T, padded):
         acc, dH, dHm = (np.zeros(T_ * N) for _ in range(3))
         ns, td, ne = np.zeros(T_ * N, dtype=np.int32), np.zeros(T_ * N, dtype=np.int32), np.zeros(T_ * N, dtype=np.uint8)
         draws = np.zeros((T_, N, D))
-        P = lambda a: None if a is None else a.ctypes.data_as(_vp)
         q = EmuNuts(model_kind=oc.DENSE_GAUSS, metric_kind=oc.DENSE, D=D, N=N, p0=P(mu), p1=P(Pm), c0=0.0, Minv=P(Minv),
                     minv_stride=0, cholU=P(cholU), eps=0.25, eps_chain=None, max_depth=4, delta_max=1000.0, sampler=0, criterion=0,
                     seed=17, offset=offset, normal_tape=None, exp_tape=None, exp_stride=0, dir_tape=None, dir_stride=0,
@@ -286,24 +269,14 @@ def test_huge_finite_poison_subset(libs, case):
 
 
 # ------------------------------------------------------------------------------------------ AddressSanitizer builds
-ASAN = {"nuts": (["-DRACE_NUTS"], 8), "lf": (["-DRACE_LF"], 5), "dense": (["-DRACE_DENSE"], 4), "glm": (["-DRACE_GLM"], 1)}
+ASAN = {"nuts": 8, "lf": 5, "dense": 4, "glm": 1}
 
 
 @pytest.mark.parametrize("name", list(ASAN))
-def test_harnesses_are_clean_under_address_sanitizer(tmp_path, name):
-    """The four tensor-pipe harnesses' small cases (tests/simt_emu/race_main.cpp) built with -fsanitize=address: host
+def test_harnesses_are_clean_under_address_sanitizer(name):
+    """The four tensor-pipe harnesses' small cases (their RACE_<NAME> mains) under AddressSanitizer: host
     buffers, the emulator's arenas and the kernels' global-memory accesses stay in bounds (the strict emulator already
     guards shared memory itself)"""
-    defs, runs = ASAN[name]
-    out = tmp_path / f"asan_{name}"
-    pr = subprocess.run(_gxx("race_main.cpp", out, *defs, "-O1", "-g", "-fsanitize=address", "-fno-omit-frame-pointer"),
-                        capture_output=True, text=True)
-    if pr.returncode != 0 and ("asan" in pr.stderr.lower() or "sanitize" in pr.stderr.lower()):
-        pytest.skip("AddressSanitizer runtime not available to g++ here")
-    assert pr.returncode == 0, pr.stderr[-3000:]
-    r = subprocess.run([str(out)], capture_output=True, text=True, timeout=900,
-                       env={**os.environ, "ASAN_OPTIONS": "detect_leaks=0"})
-    if "AddressSanitizer" in r.stderr and "ERROR: AddressSanitizer" not in r.stderr:
-        pytest.skip("AddressSanitizer cannot run in this environment: " + r.stderr.strip().splitlines()[0])
+    r = E.sanitized(name, "address")
     assert "ERROR: AddressSanitizer" not in r.stderr and r.returncode == 0, r.stderr[-3000:] + r.stdout[-500:]
-    assert r.stdout.count("rc 0") == runs
+    assert r.stdout.count("rc 0") == ASAN[name]

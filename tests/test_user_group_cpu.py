@@ -6,18 +6,15 @@ import concurrent.futures as cf
 import ctypes as C
 import importlib.util
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import ahmc_b200 as A
 from oracle import oracle_c as oc
+from tests import emu as E
+from tests.emu import P, EmuUser
 from tests.helpers import rel_err
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_vp = C.c_void_p
-P = lambda a: None if a is None else a.ctypes.data_as(_vp)
 
 FUNNEL = r'''
 #define AHMC_USER_GROUPWISE
@@ -40,67 +37,37 @@ __device__ double ahmc_user_logp_grad_group(const double* th, double* g, int D, 
 '''
 
 
-def _lib_or_skip():
-    lib = A._lib.load()
-    log = C.create_string_buffer(4096)
-    if lib.ahmc_user_source_check(FUNNEL.encode(), 0, 0, 3, log, 4096) == A._lib.ERR_UNSUPPORTED:
-        pytest.skip("libnvrtc not available here: " + log.value.decode())
-    return lib
-
-
-def _check(lib, src, kernel, metric, D):
-    log = C.create_string_buffer(8192)
-    rc = lib.ahmc_user_source_check(src.encode(), kernel, metric, D, log, 8192)
-    return rc, log.value.decode()
-
-
 def test_group_form_sources_compile_for_every_kernel_metric_and_layout():
     """kernels 0..6 (phasepoint, trajectory, static HMC, NUTS, find_good_stepsize, adaptive NUTS, adaptive static HMC) x
     Unit / Diag / Dense x D in {3, 10, 128, 512} (G = 4, 16, 32, 32), for the funnel and the logistic regression"""
-    lib = _lib_or_skip()
-    spec = importlib.util.spec_from_file_location("user_group_cost", os.path.join(ROOT, "scripts", "user_group_cost.py"))
+    lib = E.nvrtc_lib_or_skip()
+    spec = importlib.util.spec_from_file_location("user_group_cost", os.path.join(E.ROOT, "scripts", "user_group_cost.py"))
     cost = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(cost)
     jobs = [(src, kernel, metric, D) for D in (3, 10, 128, 512) for src in (FUNNEL, cost.logreg_sources(1000, D)[1])
             for kernel in range(7) for metric in (0, 1, 2)]
     with cf.ThreadPoolExecutor(max_workers=os.cpu_count() or 4) as ex:
-        results = list(ex.map(lambda j: _check(lib, *j), jobs))
+        results = list(ex.map(lambda j: E.source_check(lib, *j), jobs))
     for (src, kernel, metric, D), (rc, log) in zip(jobs, results):
         assert rc == 0, (kernel, metric, D, log[-2000:])
 
 
 def test_group_form_sources_that_do_not_compile_come_back_with_their_logs():
-    lib = _lib_or_skip()
+    lib = E.nvrtc_lib_or_skip()
     both = "#define AHMC_USER_COORDWISE\n" + FUNNEL
-    rc, log = _check(lib, both, 1, 1, 10)
+    rc, log = E.source_check(lib, both, 1, 1, 10)
     assert rc == A._lib.ERR_INVALID and "AHMC_USER_COORDWISE" in log and "AHMC_USER_GROUPWISE" in log, log
-    rc, log = _check(lib, FUNNEL.replace("return 0.0;", "return nope;"), 3, 1, 10)
+    rc, log = E.source_check(lib, FUNNEL.replace("return 0.0;", "return nope;"), 3, 1, 10)
     assert rc == A._lib.ERR_INVALID and "nope" in log and "undefined" in log, log
     with pytest.raises(A.InvalidArgument):
         A.UserTarget.check_source(both, 10)
     A.UserTarget.check_source(FUNNEL, 10)
 
 
-class EmuUser(C.Structure):
-    _fields_ = [("op", C.c_int32), ("metric_kind", C.c_int32), ("D", C.c_int32), ("N", C.c_int64), ("c0", C.c_double),
-                ("Minv", _vp), ("cholU", _vp), ("eps", C.c_double), ("n_steps", C.c_int32), ("max_depth", C.c_int32),
-                ("exp_tape", _vp), ("exp_stride", C.c_int64), ("dir_tape", _vp), ("dir_stride", C.c_int64),
-                ("th_in", _vp), ("r_in", _vp), ("g_in", _vp), ("lp_in", _vp), ("th_out", _vp), ("r_out", _vp), ("g_out", _vp),
-                ("lp_out", _vp), ("lk_out", _vp), ("steps", _vp), ("tree_depth", _vp), ("numerical", _vp), ("acc", _vp)]
-
-
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    """the group-form harness (kernel sources + emulator + the funnel as a C++ definition), compiled once"""
-    tmp = tmp_path_factory.mktemp("simt_user_group")
-    d = os.path.join(ROOT, "tests", "simt_emu")
-    out = tmp / "libuser_group_emu.so"
-    cmd = ["g++", "-O1", "-std=c++20", "-shared", "-fPIC", "-pthread", "-ffp-contract=off", "-I", os.path.join(d, "include"),
-           "-I", os.path.join(ROOT, "advancedhmc.jl_b200", "csrc"), "-I", os.path.join(ROOT, "include"),
-           os.path.join(d, "simt_emu.cpp"), os.path.join(d, "user_group_emu.cpp"), "-o", str(out)]
-    pr = subprocess.run(cmd, capture_output=True, text=True)
-    assert pr.returncode == 0, pr.stderr[-2000:]
-    return C.CDLL(str(out))
+def emu():
+    """the group-form harness (kernel sources + emulator + the funnel as a C++ definition)"""
+    return E.harness("user_group")
 
 
 MKINDS = dict(unit=oc.UNIT, diag=oc.DIAG, dense=oc.DENSE)
