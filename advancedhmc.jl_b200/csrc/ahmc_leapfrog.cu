@@ -140,9 +140,12 @@ __global__ void __launch_bounds__(kBlockThreads, min_blocks_lf<MODEL, METRIC, E>
 // integrates TWO chains, A = 2w and B = 2w + 1, one after the other, and B's loads are issued only once A's state has
 // arrived and passed its magnitude test, so they are in flight while A integrates and stores.  With one chain per warp
 // every warp of the wave issues its loads at once, DRAM serves them interleaved, and the whole wave then computes with
-// HBM idle and stores at once.  Each chain goes through run_trajectory's fast-path arithmetic (FastCoef) op for op, so
-// the results are bit-identical to the one-chain kernel.  SHARED: scalar eps and a shared M^-1, so A's coefficient
-// registers serve B too (what keeps the pair within 128 registers at E = 4); otherwise B builds its own after A is done.
+// HBM idle and stores at once.  Without SHARED each chain goes through run_trajectory's fast-path arithmetic (FastCoef)
+// op for op, bit-identical to the one-chain kernel, and B builds its own coefficients after A is done.  SHARED: scalar
+// eps and a shared M^-1, so A's coefficient registers serve B too (what keeps the pair within 128 registers at E = 4),
+// and where FastCoef::prepare_transfer allows it the warp replaces both chains' merged-step loops by one loop of the
+// same length that yields the transfer form, so B's loop no longer runs at the tail of the launch.  No CTA barrier:
+// one that made the CTA's four warps share that work measured slower than the loops it removed (DESIGN.md K1).
 // 4 blocks of 4 warps per SM (<= 128 registers): the headline 4096 chains are 2048 warps, one wave on 132 SMs.
 template <int MODEL, int METRIC, int E, bool SHARED>
 __global__ void __launch_bounds__(kBlockThreads, 4) leapfrog_pair_kernel(const LeapfrogArgs a) {
@@ -189,9 +192,14 @@ __global__ void __launch_bounds__(kBlockThreads, 4) leapfrog_pair_kernel(const L
     cload<E>(gB, (a.g_in ? a.g_in : a.th_in) + offB, l, D);
     if constexpr (METRIC == AHMC_METRIC_DIAG && !SHARED) cload<E>(miB, a.metric.Minv + a.metric.chain_stride * cB, l, D);
 
+    // SHARED: with B's loads in flight the warp derives the transfer form once for both chains (FastCoef::transfer)
+    double tu[E], td[E];
+    const bool xfer = SHARED && k.prepare_transfer(tu, td, n);
+
     bool needA, needB;
     {
-        sA |= k.steps(xA, rA, n);
+        if (xfer) k.transfer(xA, rA, tu, td);
+        else sA |= k.steps(xA, rA, n);
         double g[E], dr[E], lp, lk;
         k.last(xA, rA, g, dr, lp, lk, a.model.c0, l, D);
         sA = Grp<G>::any(sA);
@@ -200,9 +208,13 @@ __global__ void __launch_bounds__(kBlockThreads, 4) leapfrog_pair_kernel(const L
     }
     {
         if constexpr (!SHARED) k.make(miB, epsB, n, l, D);
+        // SHARED: m and w read again (L2 hits) rather than held across A, which keeps the transfer form within 128
+        // registers
+        if constexpr (SHARED) k.load_model(a.model, l, D);
         k.enter(xB, rB, gB, have_g);
         bool sB = k.bad | k.test(xB, rB);
-        sB |= k.steps(xB, rB, n);
+        if (xfer) k.transfer(xB, rB, tu, td);
+        else sB |= k.steps(xB, rB, n);
         double g[E], dr[E], lp, lk;
         k.last(xB, rB, g, dr, lp, lk, a.model.c0, l, D);
         sB = Grp<G>::any(sB);

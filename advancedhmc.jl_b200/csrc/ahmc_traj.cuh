@@ -142,6 +142,53 @@ struct FastCoef {
         }
         return s;
     }
+
+    // Transfer form of the n - 1 merged steps, for a warp whose two chains share these coefficients (K1's pair kernel
+    // with a scalar eps and a shared M^-1).  A merged step is a fixed linear map of each coordinate's (x, r),
+    // S = [[1, a], [-b, 1 - ab]] with det 1, so by Cayley-Hamilton S^m = U_(m-1) S - U_(m-2) I, U_k the Chebyshev
+    // polynomials of the second kind at tr(S)/2 = 1 - ab/2.  tu = U_(m-1) and td = U_(m-1) - U_(m-2) follow from
+    // td_k = td_(k-1) - ab tu_(k-1), tu_k = tu_(k-1) + td_k (no 2 - ab is ever formed, so nothing cancels when ab is
+    // small): one loop of the chain loop's length and cost, after which either chain's n - 1 steps are
+    // (x, r) <- (td x + a tu r, -b tu x + (td - ab tu) r), 7 ops per coordinate instead of 2(n - 1).
+    // Taken only when the whole trajectory is one proof segment (the magnitude proof tests the entry state alone, which
+    // the form of the end point does not change), n > 1, and every coordinate has 0 <= ab <= 3.  The margin: in the
+    // scaled coordinates (x/sqrt(a), r/sqrt(b)) S depends on h = sqrt(ab) only, and with cos(t) = 1 - h^2/2,
+    // N = S - cos(t) I, S^j = T_j(cos t) I + U_(j-1)(cos t) N, |T_j| <= 1, |U_(j-1)| <= 1/sin(t), |N| = h(1 + h/2), so
+    // every power of S has norm <= 1 + sqrt((2+h)/(2-h)): 2.05 at the headline's ab = 0.01, 3 + sqrt(3) at ab = 3,
+    // unbounded towards the stability edge ab = 4 or for ab < 0.  Inside it the roundings of the stepwise loop and of
+    // this form (the (tu, td) loop is the same leapfrog recurrence with a = 1, b = ab) reach the end point with that
+    // bounded gain, so the two end points differ by O(n) units in the last place of the entry state's scaled norm.
+    // The decision is uniform over the launch (every warp holds all D coordinates of the same coefficients).
+    __device__ __forceinline__ bool prepare_transfer(double (&tu)[E], double (&td)[E], int n) const {
+        bool ok = cseg == n && n > 1;
+        double ab[E];
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            ab[e] = ca[e] * cb[e];
+            ok = ok && ab[e] >= 0.0 && ab[e] <= 3.0;
+            tu[e] = 1.0;
+            td[e] = 1.0;
+        }
+        if (!__all_sync(FULL, ok)) return false;
+        for (int k = 2; k < n; ++k) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) {
+                td[e] = fma(-ab[e], tu[e], td[e]);
+                tu[e] = tu[e] + td[e];
+            }
+        }
+        return true;
+    }
+    // the n - 1 merged steps of one chain in the transfer form (tu, td: prepare_transfer)
+    __device__ __forceinline__ void transfer(double (&x)[E], double (&r)[E], const double (&tu)[E], const double (&td)[E]) const {
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+            const double pxr = ca[e] * tu[e], prx = cb[e] * tu[e], prr = fma(-cb[e], pxr, td[e]);
+            const double x0 = x[e];
+            x[e] = fma(pxr, r[e], td[e] * x0);
+            r[e] = fma(prr, r[e], -prx * x0);
+        }
+    }
     // last step: drift, gradient, half kick, energies (x back to theta).  g = x*w and dH/dr = Minv*r are recovered from the
     // per-coordinate constants as (x*b)/eps and (r*a)/eps (one extra rounding, ~1e-16 relative)
     __device__ __forceinline__ void last(double (&x)[E], double (&r)[E], double (&g)[E], double (&dr)[E], double& lp,
