@@ -53,8 +53,7 @@ struct ahmc_ctx {
     DevBuf energy_ws;     // multinomial-static per-chain energy tape
     DevBuf dense_ws;      // K4: padded Minv, norms, per-chain fallback mask
     DevBuf coop_ws;       // cooperative NUTS products: Minv and cholU with padded columns (coop_lds)
-    DevBuf split_ws;      // callback (split-step) mode workspace
-    DevBuf glm_ws;        // K6 transitions: -grad log pi of the start point
+    DevBuf split_ws;      // split-step (callback) mode and sequenced transitions (SplitWork)
     // host-buffer pipeline: upload stream, compute stream (= stream), download stream; per chunk an upload-done and a
     // kernel-done event, and one event that joins the downloads back into the compute stream
     cudaStream_t pipe[2] = {};  // upload, download
@@ -360,26 +359,35 @@ int finish_call(ahmc_ctx* ctx, Stager& st, uint32_t flags) {
 }
 
 
-// ---- split-step (callback) mode --------------------------------------------------------------------------------
+// D x N doubles from src (leading dimension lds) to dst (ldd) on the context stream; nothing if they are the same array
+cudaError_t copy_chains(ahmc_ctx* ctx, double* dst, int64_t ldd, const double* src, int64_t lds, int32_t D, int64_t N) {
+    if (dst == src) return cudaSuccess;
+    return cudaMemcpy2DAsync(dst, (size_t)ldd * 8, src, (size_t)lds * 8, (size_t)D * 8, (size_t)N, cudaMemcpyDeviceToDevice,
+                             ctx->stream);
+}
+
+// ---- split-step (callback) mode and sequenced transitions ------------------------------------------------------
 struct SplitWork {
-    double* cb_lp;
+    double* cb_lp;           // the callback's outputs: lp[N], grad[ld x N]
     double* cb_grad;
-    double* r0;
+    double* r0;              // a transition's refreshed momentum (D x N) and its kinetic energy
     double* lk0;
-    uint32_t* status;
-    int32_t* steps;
-    int* flag;
+    uint32_t* status;        // per-chain status of a trajectory whose caller passes none
+    int* flag;               // set when a chain turns non-finite in a step (COMPAT_BREAK_ALL)
+    double *th0, *g0, *lp0;  // a transition's start point (D x N), when it is copied aside (`start`), else nullptr
 };
 
-int split_workspace(ahmc_ctx* ctx, int32_t D, int64_t N, int64_t ld, SplitWork* w) {
+int split_workspace(ahmc_ctx* ctx, int32_t D, int64_t N, int64_t ld, bool start, SplitWork* w) {
     return carve(ctx, ctx->split_ws, "the split-step workspace", [&](Carver& c) {
         w->cb_lp = c.take<double>((size_t)N);
         w->cb_grad = c.take<double>((size_t)ld * N);
         w->r0 = c.take<double>((size_t)D * N);
         w->lk0 = c.take<double>((size_t)N);
         w->status = c.take<uint32_t>((size_t)N);
-        w->steps = c.take<int32_t>((size_t)N);
         w->flag = c.take<int>(1);
+        w->th0 = c.take<double>((size_t)D * N, start);
+        w->g0 = c.take<double>((size_t)D * N, start);
+        w->lp0 = c.take<double>((size_t)N, start);
     });
 }
 
@@ -391,33 +399,39 @@ int call_user(ahmc_ctx* ctx, const ahmc_model* model, const double* th, double* 
     return AHMC_OK;
 }
 
-// n leapfrog steps in split mode on DEVICE work arrays (th, r, g, lp, lk[, dr]); status/steps are device arrays
-int split_trajectory(ahmc_ctx* ctx, const ahmc_model* model, const MetricDev& md, int32_t D, int64_t N, double eps,
-                     const double* eps_chain, int n_abs, int fwd, double temper_alpha, double* th, double* r, double* g,
-                     double* lp, double* lk, double* dr, int64_t ld, uint32_t* status, int32_t* steps, const SplitWork& w,
-                     bool compat, int* nl) {
+// lf.n_steps leapfrog steps in split mode (DEVICE pointers; w from split_workspace at lf.ld_out): the work state is the
+// output phase point, which starts as a copy of the input one.  Per step a kick_drift kernel, the user closure and a
+// kick_energy kernel.
+int split_trajectory(ahmc_ctx* ctx, const ahmc_model* model, const LeapfrogArgs& lf, const SplitWork& w, bool compat, int* nl) {
+    const int D = lf.D, n = lf.n_steps;
+    const long long N = lf.N, ld = lf.ld_out;
+    CU(copy_chains(ctx, lf.th_out, ld, lf.th_in, lf.ld_in, D, N));
+    CU(copy_chains(ctx, lf.r_out, ld, lf.r_in, lf.ld_in, D, N));
+    CU(copy_chains(ctx, lf.g_out, ld, lf.g_in, lf.ld_in, D, N));
+    uint32_t* status = lf.status ? lf.status : w.status;
     CU(cudaMemsetAsync(status, 0, (size_t)N * 4, ctx->stream));
-    if (steps) CU(cudaMemsetAsync(steps, 0, (size_t)N * 4, ctx->stream));
+    if (lf.steps_done) CU(cudaMemsetAsync(lf.steps_done, 0, (size_t)N * 4, ctx->stream));
     CU(cudaMemsetAsync(w.flag, 0, sizeof(int), ctx->stream));
-    const double sa = temper_alpha > 0.0 ? sqrt(temper_alpha) : 1.0;
-    for (int i = 1; i <= n_abs; ++i) {
+    const double ta = lf.temper_alpha;
+    const double sa = ta > 0.0 ? sqrt(ta) : 1.0;
+    for (int i = 1; i <= n; ++i) {
         SplitArgs a{};
-        a.metric = md;
+        a.metric = lf.metric;
         a.D = D;
         a.N = N;
-        a.eps = eps;
-        a.eps_chain = eps_chain;
-        a.fwd = fwd;
-        a.mul = temper_alpha > 0.0 ? ((2 * (i - 1) + 1 <= n_abs) ? sa : 1.0 / sa) : 1.0;
+        a.eps = lf.eps;
+        a.eps_chain = lf.eps_chain;
+        a.fwd = lf.fwd;
+        a.mul = ta > 0.0 ? ((2 * (i - 1) + 1 <= n) ? sa : 1.0 / sa) : 1.0;
         a.step_index = i;
-        a.th = th; a.r = r; a.g = g; a.lp = lp; a.lk = lk; a.dr = dr;
+        a.th = lf.th_out; a.r = lf.r_out; a.g = lf.g_out; a.lp = lf.lp_out; a.lk = lf.lk_out; a.dr = lf.dr_out;
         a.cb_lp = w.cb_lp; a.cb_grad = w.cb_grad;
         a.ld = ld;
-        a.status = status; a.steps_done = steps; a.any_nonfinite = w.flag;
+        a.status = status; a.steps_done = lf.steps_done; a.any_nonfinite = w.flag;
         CU(launch_kick_drift(a, ctx->stream, nl));
-        int rc = call_user(ctx, model, th, w.cb_lp, w.cb_grad, D, N, ld);
+        int rc = call_user(ctx, model, lf.th_out, w.cb_lp, w.cb_grad, D, N, ld);
         if (rc) return rc;
-        a.mul = temper_alpha > 0.0 ? ((2 * (i - 1) + 2 <= n_abs) ? sa : 1.0 / sa) : 1.0;
+        a.mul = ta > 0.0 ? ((2 * (i - 1) + 2 <= n) ? sa : 1.0 / sa) : 1.0;
         CU(launch_kick_energy(a, ctx->stream, nl));
         if (compat) {  // reference quirk Q1: first non-finite chain stops everyone (hamiltonian.jl:141-142)
             int f = 0;
@@ -430,24 +444,22 @@ int split_trajectory(ahmc_ctx* ctx, const ahmc_model* model, const MetricDev& md
 }
 
 // can the tiled DMMA trajectory (K4) run this target and metric?  A Gaussian target with a GEMM-shaped operator (dense
-// metric and/or dense-Gaussian target), one M^-1 shared by all chains, no EXACT_CHECKS, and a tile shape for D
-bool dense_tile_eligible(const ahmc_model* model, const MetricDev& metric, uint32_t flags, int32_t D) {
+// metric and/or dense-Gaussian target), one M^-1 shared by all chains, no EXACT_CHECKS / COMPAT_BREAK_ALL, and a tile
+// shape for D
+bool dense_tile_eligible(const ahmc_model* model, const MetricDev& metric, uint32_t flags) {
     const bool gauss = model->kind == AHMC_MODEL_STD_NORMAL || model->kind == AHMC_MODEL_DIAG_GAUSS ||
                        model->kind == AHMC_MODEL_DENSE_GAUSS;
     const bool has_dense = model->kind == AHMC_MODEL_DENSE_GAUSS || metric.kind == AHMC_METRIC_DENSE;
     int Dp, RB, CB;
-    return gauss && has_dense && metric.chain_stride == 0 && !(flags & AHMC_FLAG_EXACT_CHECKS) &&
-           dense_tile_shape(D, &Dp, &RB, &CB) && (model->kind != AHMC_MODEL_DENSE_GAUSS || model->d_p1_pad);
+    return gauss && has_dense && metric.chain_stride == 0 && !(flags & (AHMC_FLAG_EXACT_CHECKS | AHMC_FLAG_COMPAT_BREAK_ALL)) &&
+           dense_tile_shape(model->D, &Dp, &RB, &CB) && (model->kind != AHMC_MODEL_DENSE_GAUSS || model->d_p1_pad);
 }
 
-// K4 dispatch: GEMM-shaped operators (dense metric and/or dense-Gaussian target) -> tiled DMMA kernel; chains of tiles it
-// declines (magnitude proof not met) are redone by the exact warp-per-chain kernel from the untouched inputs.
-// `a` holds DEVICE pointers.  Returns 1 if handled, 0 if the configuration is not eligible, < 0 on error.
-int try_dense_trajectory(ahmc_ctx* ctx, const ahmc_model* model, LeapfrogArgs& a, int n_abs, double eps, double temper_alpha,
-                         bool compat, int* nl) {
+// K4: GEMM-shaped operators (dense metric and/or dense-Gaussian target) -> tiled DMMA kernel; chains of tiles it declines
+// (magnitude proof not met) are redone by the exact warp-per-chain kernel from the untouched inputs.  DEVICE pointers.
+int dense_trajectory(ahmc_ctx* ctx, const ahmc_model* model, const LeapfrogArgs& a, int* nl) {
     const int D = a.D;
     const long long N = a.N;
-    if (!dense_tile_eligible(model, a.metric, a.flags, D) || compat || !a.g_in || temper_alpha > 0.0) return 0;
     int Dp, RB, CB;
     dense_tile_shape(D, &Dp, &RB, &CB);
     double *Mpad, *norms;
@@ -478,66 +490,20 @@ int try_dense_trajectory(ahmc_ctx* ctx, const ahmc_model* model, LeapfrogArgs& a
     }
     *nl += 1;
     h.norms = norms;
-    h.eps = eps; h.eps_chain = a.eps_chain; h.n_steps = n_abs; h.fwd = a.fwd;
+    h.eps = a.eps; h.eps_chain = a.eps_chain; h.n_steps = a.n_steps; h.fwd = a.fwd;
     h.th_in = a.th_in; h.r_in = a.r_in; h.g_in = a.g_in; h.ld_in = a.ld_in;
     h.th_out = a.th_out; h.r_out = a.r_out; h.g_out = a.g_out; h.dr_out = a.dr_out;
     h.lp_out = a.lp_out; h.lk_out = a.lk_out; h.ld_out = a.ld_out;
     h.status = a.status; h.steps_done = a.steps_done; h.need_exact = mask;
     CU(launch_dense_traj(h, ctx->stream, nl));
     LeapfrogArgs b = a;
-    b.n_steps = n_abs;
     b.only_mask = mask;
-    b.min_break = nullptr;
     CU(launch_leapfrog(b, ctx->stream, nl));
-    return 1;
-}
-// hmc_kernel's transition, unfused, for what it cannot run itself (callback targets, the tiled DMMA trajectory):
-// refresh -> kinetic energy -> start point into z_out -> `trajectory(w)` in place on z_out (< 0 on error) -> MH select.
-// `h` holds DEVICE pointers.
-template <class Trajectory>
-static int unfused_transition(ahmc_ctx* ctx, const HmcArgs& h, int* nl, Trajectory&& trajectory) {
-    const LeapfrogArgs& a = h.lf;
-    const int D = a.D;
-    const long long N = a.N;
-    SplitWork w;
-    int rc = split_workspace(ctx, D, N, a.ld_out, &w);
-    if (rc) return rc;
-    if (h.refresh) {
-        MomentumArgs ma{};
-        ma.metric = a.metric; ma.D = D; ma.N = N; ma.seed = h.rng.seed; ma.offset = h.rng.offset;
-        ma.normal_tape = h.rng.normal_tape; ma.r = w.r0; ma.ld = D;
-        CU(launch_rand_momentum(ma, ctx->stream, nl));
-    } else {
-        CU(cudaMemcpy2DAsync(w.r0, (size_t)D * 8, a.r_in, (size_t)a.ld_in * 8, (size_t)D * 8, (size_t)N,
-                             cudaMemcpyDeviceToDevice, ctx->stream));
-    }
-    SplitArgs k0{};  // lk0 = neg kinetic energy of the refreshed momentum
-    k0.metric = a.metric; k0.D = D; k0.N = N; k0.fwd = 1; k0.mul = 1.0; k0.no_kick = 1;
-    k0.r = w.r0; k0.lk = w.lk0; k0.ld = D;
-    CU(launch_kick_energy(k0, ctx->stream, nl));
-    auto cp = [&](double* dst, const double* src, int64_t lds) -> cudaError_t {
-        if (dst == src) return cudaSuccess;
-        return cudaMemcpy2DAsync(dst, (size_t)a.ld_out * 8, src, (size_t)lds * 8, (size_t)D * 8, (size_t)N,
-                                 cudaMemcpyDeviceToDevice, ctx->stream);
-    };
-    if (a.th_out == a.th_in)
-        return fail(ctx, AHMC_ERR_INVALID, "callback-mode transitions need z_out distinct from z_in (the start point is re-read on rejection)");
-    CU(cp(a.th_out, a.th_in, a.ld_in));
-    CU(cp(a.g_out, a.g_in, a.ld_in));
-    CU(cp(a.r_out, w.r0, D));
-    if ((rc = trajectory(w)) < 0) return rc;
-    MhArgs m{};
-    m.D = D; m.N = N; m.n_steps = a.n_steps;
-    m.th0 = a.th_in; m.g0 = a.g_in; m.lp0 = a.lp_in; m.ld0 = a.ld_in;
-    m.r0 = w.r0; m.lk0 = w.lk0;
-    m.th = a.th_out; m.r = a.r_out; m.g = a.g_out; m.lp = a.lp_out; m.lk = a.lk_out; m.ld = a.ld_out;
-    m.rng = h.rng; m.st = h.st;
-    CU(launch_mh_select(m, ctx->stream, nl));
     return AHMC_OK;
 }
 
 // can the chain-tile kernel (K6) run this call?  A GLM target, device buffers, a Unit or Diag metric (shared or per
-// chain), no EXACT_CHECKS, and a tile shape for (D, n)
+// chain), no EXACT_CHECKS / COMPAT_BREAK_ALL, and a tile shape for (D, n)
 bool glm_tile_eligible(const ahmc_model* model, const MetricDev& metric, uint32_t flags) {
     int RB, CB, nc, stages;
     size_t sm;
@@ -555,50 +521,71 @@ GlmArgs glm_args(const ahmc_model* model, const MetricDev& metric, int64_t N) {
     g.chain_stride = metric.chain_stride;
     return g;
 }
-// K6 dispatch, as try_dense_trajectory: 1 if handled, 0 if the call is not eligible, < 0 on error.  `a`: DEVICE pointers.
-int try_glm_trajectory(ahmc_ctx* ctx, const ahmc_model* model, const LeapfrogArgs& a, int n_abs, double eps, double temper_alpha,
-                       int* nl) {
-    if (!glm_tile_eligible(model, a.metric, a.flags) || temper_alpha > 0.0) return 0;
+// K6: the GLM target's trajectory on the chain-tile kernel.  DEVICE pointers.
+int glm_trajectory(ahmc_ctx* ctx, const ahmc_model* model, const LeapfrogArgs& a, int* nl) {
     GlmArgs g = glm_args(model, a.metric, a.N);
-    g.eps = eps; g.eps_chain = a.eps_chain; g.n_steps = n_abs; g.fwd = a.fwd;
+    g.eps = a.eps; g.eps_chain = a.eps_chain; g.n_steps = a.n_steps; g.fwd = a.fwd;
     g.th_in = a.th_in; g.r_in = a.r_in; g.g_in = a.g_in; g.ld_in = a.ld_in;
     g.th_out = a.th_out; g.r_out = a.r_out; g.g_out = a.g_out; g.dr_out = a.dr_out;
     g.lp_out = a.lp_out; g.lk_out = a.lk_out; g.ld_out = a.ld_out;
     g.status = a.status; g.steps_done = a.steps_done;
     CU(launch_glm_traj(g, ctx->stream, nl));
-    return 1;
+    return AHMC_OK;
 }
-int glm_start_workspace(ahmc_ctx* ctx, size_t bytes, double** out) {  // -grad log pi of a transition's start point
-    int rc = ensure(ctx, ctx->glm_ws, bytes, "the GLM start-point workspace");
-    *out = (double*)ctx->glm_ws.p;
-    return rc;
+
+// The engine that integrates a call's trajectory, for ahmc_leapfrog_f64 and the static HMC transitions (hmc_impl adds
+// conditions of its own before K4 or K6 runs a transition).
+enum class Engine {
+    Dense,  // K4, dense_trajectory
+    Glm,    // K6, glm_trajectory
+    Split,  // callback target, split_trajectory
+    Fused,  // the register-resident kernels (K1 leapfrog, hmc_kernel), D > 512 and run-time compiled forms included
+};
+Engine trajectory_engine(const ahmc_model* model, const MetricDev& metric, uint32_t flags, double temper_alpha, bool has_grad) {
+    if (model->kind == AHMC_MODEL_CALLBACK) return Engine::Split;
+    if (temper_alpha > 0.0) return Engine::Fused;  // K4 and K6 integrate plain Leapfrog
+    if (dense_tile_eligible(model, metric, flags) && has_grad) return Engine::Dense;  // K4 reads the start point's gradient
+    if (glm_tile_eligible(model, metric, flags)) return Engine::Glm;
+    return Engine::Fused;
 }
-// Static transitions of a GLM target on the tile kernel: per transition refresh -> kinetic energy -> K6 in place on z_out
-// -> MH select, enqueued back to back without a host synchronisation; transition t draws at Philox offset offset + t,
-// starts from transition t - 1's z_out and writes row t of `draws` and of the statistics.  The start point of each
-// transition is kept in the split workspace (a rejection re-reads it), so z_out may alias z_in.
-int glm_transitions(ahmc_ctx* ctx, const ahmc_model* model, const HmcArgs& h, int* nl) {
+// the trajectory of engine `e` (not Fused) from lf's inputs to its outputs; `w` serves the split-step engine
+int run_trajectory(ahmc_ctx* ctx, const ahmc_model* model, Engine e, const LeapfrogArgs& lf, const SplitWork& w, bool compat,
+                   int* nl) {
+    if (e == Engine::Dense) return dense_trajectory(ctx, model, lf, nl);
+    if (e == Engine::Glm) return glm_trajectory(ctx, model, lf, nl);
+    return split_trajectory(ctx, model, lf, w, compat, nl);
+}
+
+// row `off` / N of statistics arrays that hold N entries per transition
+StatsDev stats_row(StatsDev s, size_t off) {
+    auto at = [off](auto* p) { return p ? p + off : p; };
+    s.n_steps = at(s.n_steps);
+    s.is_accept = at(s.is_accept);
+    s.acceptance_rate = at(s.acceptance_rate);
+    s.log_density = at(s.log_density);
+    s.hamiltonian_energy = at(s.hamiltonian_energy);
+    s.hamiltonian_energy_error = at(s.hamiltonian_energy_error);
+    s.max_hamiltonian_energy_error = at(s.max_hamiltonian_energy_error);
+    s.tree_depth = at(s.tree_depth);
+    s.numerical_error = at(s.numerical_error);
+    return s;
+}
+
+// hmc_kernel's static transitions, one kernel per stage, for the engines it cannot fuse (K4, K6, split-step): per
+// transition refresh -> kinetic energy -> trajectory from the start point into z_out -> MH select, enqueued back to back
+// (only a callback target's closure may synchronise).  Transition t draws at Philox offset offset + t, starts from z_in
+// (t = 0) or from transition t - 1's z_out, and writes row t of `draws` and of the statistics.  `h`: DEVICE pointers.
+int sequenced_transitions(ahmc_ctx* ctx, const ahmc_model* model, Engine e, const HmcArgs& h, int* nl) {
     const LeapfrogArgs& a = h.lf;
     const int D = a.D;
     const long long N = a.N;
+    const bool alias = a.th_out == a.th_in;
     SplitWork w;
-    int rc = split_workspace(ctx, D, N, D, &w);
+    int rc = split_workspace(ctx, D, N, a.ld_out, h.n_transitions > 1 || alias, &w);
     if (rc) return rc;
-    double *th0 = w.cb_grad, *g0, *lp0 = w.cb_lp;  // start point: theta in cb_grad, -grad in glm_ws, lp in cb_lp
-    if ((rc = glm_start_workspace(ctx, (size_t)D * N * sizeof(double), &g0))) return rc;
-    auto cp = [&](double* dst, long long ldd, const double* src, long long lds) -> cudaError_t {
-        if (dst == src) return cudaSuccess;
-        return cudaMemcpy2DAsync(dst, (size_t)ldd * 8, src, (size_t)lds * 8, (size_t)D * 8, (size_t)N, cudaMemcpyDeviceToDevice,
-                                 ctx->stream);
-    };
     for (int t = 0; t < h.n_transitions; ++t) {
-        const double* th = t ? a.th_out : a.th_in;
-        const double* gr = t ? a.g_out : a.g_in;
-        const double* rr = t ? a.r_out : a.r_in;
-        const long long ld = t ? a.ld_out : a.ld_in;
-        CU(cp(th0, D, th, ld));
-        CU(cp(g0, D, gr, ld));
-        CU(cudaMemcpyAsync(lp0, t ? a.lp_out : a.lp_in, (size_t)N * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+        const double *th0 = t ? a.th_out : a.th_in, *g0 = t ? a.g_out : a.g_in, *lp0 = t ? a.lp_out : a.lp_in;
+        long long ld0 = t ? a.ld_out : a.ld_in;
         RngDev rng = h.rng;
         rng.offset += (uint64_t)t;
         if (h.refresh) {
@@ -607,33 +594,42 @@ int glm_transitions(ahmc_ctx* ctx, const ahmc_model* model, const HmcArgs& h, in
             ma.normal_tape = rng.normal_tape; ma.r = w.r0; ma.ld = D;
             CU(launch_rand_momentum(ma, ctx->stream, nl));
         } else {
-            CU(cp(w.r0, D, rr, ld));
+            CU(copy_chains(ctx, w.r0, D, t ? a.r_out : a.r_in, ld0, D, N));
         }
         SplitArgs k0{};  // lk0 = neg kinetic energy of the refreshed momentum
         k0.metric = a.metric; k0.D = D; k0.N = N; k0.fwd = 1; k0.mul = 1.0; k0.no_kick = 1;
         k0.r = w.r0; k0.lk = w.lk0; k0.ld = D;
         CU(launch_kick_energy(k0, ctx->stream, nl));
+        // MH select re-reads the start point after the trajectory has written z_out: when z_out holds it (t > 0) or
+        // aliases it, it is copied aside first
+        if (t || alias) {
+            CU(copy_chains(ctx, w.th0, D, th0, ld0, D, N));
+            CU(copy_chains(ctx, w.g0, D, g0, ld0, D, N));
+            CU(cudaMemcpyAsync(w.lp0, lp0, (size_t)N * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+            th0 = w.th0; g0 = w.g0; lp0 = w.lp0; ld0 = D;
+        }
         LeapfrogArgs lf = a;
-        lf.th_in = th0; lf.g_in = g0; lf.r_in = w.r0; lf.ld_in = D;
-        lf.status = nullptr; lf.steps_done = nullptr; lf.dr_out = nullptr;
-        if ((rc = try_glm_trajectory(ctx, model, lf, a.n_steps, a.eps, 0.0, nl)) < 0) return rc;
+        lf.temper_alpha = h.rng.temper_alpha;
+        if (ld0 == D) {
+            lf.th_in = th0; lf.r_in = w.r0; lf.g_in = g0; lf.ld_in = D;
+        } else {  // the trajectory reads theta, r and -grad at one leading dimension, and r0's is D: it starts from a
+                  // copy of the start point in z_out
+            CU(copy_chains(ctx, a.th_out, a.ld_out, th0, ld0, D, N));
+            CU(copy_chains(ctx, a.g_out, a.ld_out, g0, ld0, D, N));
+            CU(copy_chains(ctx, a.r_out, a.ld_out, w.r0, D, D, N));
+            lf.th_in = a.th_out; lf.r_in = a.r_out; lf.g_in = a.g_out; lf.ld_in = a.ld_out;
+        }
+        if ((rc = run_trajectory(ctx, model, e, lf, w, false, nl))) return rc;
         MhArgs m{};
         m.D = D; m.N = N; m.n_steps = a.n_steps;
-        m.th0 = th0; m.g0 = g0; m.lp0 = lp0; m.ld0 = D;
+        m.th0 = th0; m.g0 = g0; m.lp0 = lp0; m.ld0 = ld0;
         m.r0 = w.r0; m.lk0 = w.lk0;
         m.th = a.th_out; m.r = a.r_out; m.g = a.g_out; m.lp = a.lp_out; m.lk = a.lk_out; m.ld = a.ld_out;
         m.rng = rng;
-        m.st = h.st;
-        const size_t so = (size_t)t * N;
-        if (m.st.n_steps) m.st.n_steps += so;
-        if (m.st.is_accept) m.st.is_accept += so;
-        if (m.st.acceptance_rate) m.st.acceptance_rate += so;
-        if (m.st.log_density) m.st.log_density += so;
-        if (m.st.hamiltonian_energy) m.st.hamiltonian_energy += so;
-        if (m.st.hamiltonian_energy_error) m.st.hamiltonian_energy_error += so;
-        if (m.st.numerical_error) m.st.numerical_error += so;
+        const size_t row = (size_t)t * N;
+        m.st = stats_row(h.st, row);
         CU(launch_mh_select(m, ctx->stream, nl));
-        if (h.draws) CU(cp(h.draws + so * D, D, a.th_out, a.ld_out));
+        if (h.draws) CU(copy_chains(ctx, h.draws + row * D, D, a.th_out, a.ld_out, D, N));
     }
     return AHMC_OK;
 }
@@ -693,7 +689,7 @@ int ahmc_destroy(ahmc_ctx* ctx) {
     DeviceGuard g(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     cudaFree(ctx->d_min_break);
-    for (DevBuf* b : {&ctx->arena, &ctx->chain_ws, &ctx->summary_ws, &ctx->energy_ws, &ctx->dense_ws, &ctx->coop_ws, &ctx->split_ws, &ctx->glm_ws})
+    for (DevBuf* b : {&ctx->arena, &ctx->chain_ws, &ctx->summary_ws, &ctx->energy_ws, &ctx->dense_ws, &ctx->coop_ws, &ctx->split_ws})
         cudaFree(b->p);
     for (cudaStream_t s : ctx->pipe)
         if (s) cudaStreamDestroy(s);
@@ -943,7 +939,7 @@ int ahmc_phasepoint_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metri
     int nl = 0;
     if (model->kind == AHMC_MODEL_CALLBACK) {  // user closure, then the metric half of phasepoint
         SplitWork w;
-        if ((rc = split_workspace(ctx, D, N, z->ld, &w))) return rc;
+        if ((rc = split_workspace(ctx, D, N, z->ld, false, &w))) return rc;
         if ((rc = call_user(ctx, model, a.th, w.cb_lp, w.cb_grad, D, N, z->ld))) return rc;
         SplitArgs sa{};
         sa.metric = a.metric; sa.D = D; sa.N = N; sa.fwd = 1; sa.mul = 1.0; sa.no_kick = 1;
@@ -1270,34 +1266,13 @@ int ahmc_leapfrog_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric*
     const bool compat = flags & AHMC_FLAG_COMPAT_BREAK_ALL;
     a.min_break = nullptr;
     a.only_mask = nullptr;
-    {
-        int nl2 = 0;
-        rc = try_dense_trajectory(ctx, model, a, n_abs, eps, temper_alpha, compat, &nl2);
-        if (rc < 0) return rc;
-        if (rc == 0) rc = try_glm_trajectory(ctx, model, a, n_abs, eps, temper_alpha, &nl2);
-        if (rc < 0) return rc;
-        if (rc == 1) {
-            ctx->launches += nl2;
-            return finish_call(ctx, st, flags);
-        }
-    }
-    if (model->kind == AHMC_MODEL_CALLBACK) {
-        // split-step mode: the work state is the OUTPUT phase point; two small kernels + the user closure per step
-        SplitWork w;
-        if ((rc = split_workspace(ctx, D, N, z_out->ld, &w))) return rc;
-        auto cp = [&](double* dst, const double* src) -> cudaError_t {
-            if (dst == src) return cudaSuccess;
-            return cudaMemcpy2DAsync(dst, (size_t)a.ld_out * 8, src, (size_t)a.ld_in * 8, (size_t)D * 8, (size_t)N,
-                                     cudaMemcpyDeviceToDevice, ctx->stream);
-        };
-        CU(cp(a.th_out, a.th_in));
-        CU(cp(a.r_out, a.r_in));
-        CU(cp(a.g_out, a.g_in));
-        int nl2 = 0;
-        rc = split_trajectory(ctx, model, a.metric, D, N, eps, a.eps_chain, n_abs, a.fwd, temper_alpha, a.th_out, a.r_out,
-                              a.g_out, a.lp_out, a.lk_out, a.dr_out, a.ld_out, a.status ? a.status : w.status,
-                              a.steps_done, w, compat, &nl2);
-        ctx->launches += nl2;
+    const Engine e = trajectory_engine(model, a.metric, flags, temper_alpha, a.g_in != nullptr);
+    if (e != Engine::Fused) {
+        SplitWork w{};
+        if (e == Engine::Split && (rc = split_workspace(ctx, D, N, z_out->ld, false, &w))) return rc;
+        int nl = 0;
+        rc = run_trajectory(ctx, model, e, a, w, compat, &nl);
+        ctx->launches += nl;
         if (rc) return rc;
         return finish_call(ctx, st, flags);
     }
@@ -1565,30 +1540,17 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
     });
     if (rc) return rc;
     int nl = 0;
-    if (model->kind == AHMC_MODEL_CALLBACK) {
-        rc = unfused_transition(ctx, h, &nl, [&](const SplitWork& w) {
-            return split_trajectory(ctx, model, a.metric, D, N, eps, a.eps_chain, n_steps, 1, h.rng.temper_alpha, a.th_out, a.r_out,
-                                    a.g_out, a.lp_out, a.lk_out, nullptr, a.ld_out, w.status, w.steps, w, false, &nl);
-        });
+    Engine e = trajectory_engine(model, a.metric, flags, h.rng.temper_alpha, true);
+    // K4 and K6 run a transition in stages (sequenced_transitions), whose momentum refresh is a full one; in-launch
+    // adaptation is built into hmc_kernel only
+    if ((e == Engine::Dense || e == Engine::Glm) && (cfg || h.rng.partial_alpha != 0.0)) e = Engine::Fused;
+    // K4 serves one transition into a separate z_out, without draws.  Sampling launches (several transitions, draws, or
+    // z_out = z_in to chain calls in place) stay on hmc_kernel, so that a run's draws do not depend on how it is split
+    // into launches: K4's DMMA products round differently from hmc_kernel's
+    if (e == Engine::Dense && (n_transitions > 1 || a.th_out == a.th_in || draws)) e = Engine::Fused;
+    if (e != Engine::Fused) {
+        rc = sequenced_transitions(ctx, model, e, h, &nl);
         if (rc) return rc;
-        ctx->launches += nl;
-        return finish_call(ctx, st, flags);
-    }
-    if (!cfg && n_transitions == 1 && a.th_out != a.th_in && h.rng.partial_alpha == 0.0 && !(h.rng.temper_alpha > 0.0) && !draws &&
-        dense_tile_eligible(model, a.metric, flags, D)) {
-        // GEMM-shaped operators: the tiled DMMA trajectory, in place on z_out
-        rc = unfused_transition(ctx, h, &nl, [&](const SplitWork&) {
-            LeapfrogArgs t = a;
-            t.th_in = a.th_out; t.r_in = a.r_out; t.g_in = a.g_out; t.ld_in = a.ld_out;
-            t.status = nullptr; t.steps_done = nullptr; t.only_mask = nullptr; t.min_break = nullptr;
-            return try_dense_trajectory(ctx, model, t, n_steps, eps, 0.0, false, &nl);
-        });
-        if (rc) return rc;
-        ctx->launches += nl;
-        return finish_call(ctx, st, flags);
-    }
-    if (!cfg && h.rng.partial_alpha == 0.0 && !(h.rng.temper_alpha > 0.0) && glm_tile_eligible(model, a.metric, flags)) {
-        if ((rc = glm_transitions(ctx, model, h, &nl))) return rc;
         ctx->launches += nl;
         return finish_call(ctx, st, flags);
     }

@@ -275,8 +275,12 @@ def test_full_size_properties():
 
 # ------------------------------------------------------------------------------------------------ transitions
 @pytest.mark.parametrize("model,metric,D", [("diag_gauss", "diag", 128), ("std_normal", "unit", 10),
-                                            ("funnel", "diag", 20), ("dense_gauss", "dense", 12)])
+                                            ("funnel", "diag", 20), ("dense_gauss", "dense", 12),
+                                            ("dense_gauss", "diag", 24), ("diag_gauss", "dense", 64)])
 def test_hmc_transition_vs_oracle_with_tapes(model, metric, D):
+    """GEMM-shaped operators (dense-Gaussian target or Dense metric) run on the tiled fp64-MMA trajectory (K4) in stages:
+    refresh, kinetic energy, the norms of M^-1 and of the target (a dense-Gaussian target's is stored with its padded
+    precision), the tile kernel, its exact fallback and the Metropolis select.  Every other case is one hmc_kernel launch."""
     rng = np.random.default_rng(D)
     N = 301
     p0 = p1 = Minv = None
@@ -299,7 +303,12 @@ def test_hmc_transition_vs_oracle_with_tapes(model, metric, D):
     h = A.Hamiltonian(make_metric(metric, Minv, D), make_target(model, D, p0, p1, 0.0))
     z0 = A.phasepoint(h, T(th), T(np.zeros((D, N))))
     tau = A.Trajectory(A.EndPointTS, A.Leapfrog(eps), A.FixedNSteps(L))
-    tr = A.transition(A.TapeRNG(normal=T(nt), exp=torch.as_tensor(et, device=DEV)), h, A.HMCKernel(tau), z0)
+    tape = A.TapeRNG(normal=T(nt), exp=torch.as_tensor(et, device=DEV))
+    ctx = A.get_context(0)
+    l0 = ctx.launches
+    tr = A.transition(tape, h, A.HMCKernel(tau), z0)
+    k4 = model == "dense_gauss" or metric == "dense"
+    assert ctx.launches - l0 == (1 if not k4 else 6 if model == "dense_gauss" else 7)
     acc = F(tr.stat["is_accept"]).astype(bool)
     assert 0 < acc.sum() < N
     assert (acc == so.is_accept.astype(bool)).all()
