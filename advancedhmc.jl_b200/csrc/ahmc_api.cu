@@ -176,11 +176,19 @@ int carve(ahmc_ctx* ctx, DevBuf& b, const char* what, Layout&& layout) {
     return AHMC_OK;
 }
 
+// `rows` rows of `width` bytes, `pitch` bytes apart (the D rows of each of N chains at leading dimension ld): one
+// contiguous copy when there is no gap between rows, else a 2-D copy that leaves the bytes between rows alone
+cudaError_t copy_rows(void* dst, const void* src, size_t width, size_t pitch, size_t rows, cudaMemcpyKind kind,
+                      cudaStream_t s) {
+    if (width == pitch || rows == 1) return cudaMemcpyAsync(dst, src, width + pitch * (rows - 1), kind, s);
+    return cudaMemcpy2DAsync(dst, pitch, src, pitch, width, rows, kind, s);
+}
+
 // Maps caller arrays to device arrays.  An entry point describes its arrays once, in a bind function (of Stager&) that
-// calls in / out / inout for each and that neither launches kernels nor reads staged data; stage() runs it.
-// Device-pointer mode: one pass, the identity.  HOST_BUFFERS mode: a first pass only measures the arrays, the context
-// arena grows to fit, and a second pass carves them out of it and enqueues the uploads on the context stream;
-// finish() enqueues the downloads.  The first failed copy is kept and returned by stage().
+// calls in / out / inout for each (in2d / out2d for a D x N field) and that neither launches kernels nor reads staged
+// data; stage() runs it.  Device-pointer mode: one pass, the identity.  HOST_BUFFERS mode: a first pass only measures
+// the arrays, the context arena grows to fit, and a second pass carves them out of it and enqueues the uploads on the
+// context stream; finish() enqueues the downloads.  The first failed copy is kept and returned by stage().
 class Stager {
 public:
     Stager(ahmc_ctx* c, bool host) : ctx_(c), host_(host) {}
@@ -202,38 +210,65 @@ public:
     }
     template <class T>
     void in(const T* h, size_t count, const T** d) {
-        *d = map(h, count, true, false);
+        *d = map(h, Span::flat(count), true, false);
     }
     template <class T>
     void out(T* h, size_t count, T** d) {
-        *d = map(h, count, false, true);
+        *d = map(h, Span::flat(count), false, true);
     }
     template <class T>
     void inout(T* h, size_t count, T** d) {  // copied in now, copied back at finish
-        *d = map(h, count, true, true);
+        *d = map(h, Span::flat(count), true, true);
+    }
+    // a D x N field at leading dimension ld (out2d: `blocks` of them, `block_stride` doubles apart -- a trajectory's
+    // steps).  The device copy keeps the caller's layout and only rows d < D are copied: the caller's padding rows
+    // D..ld-1 are neither read nor written, and the array needs no more than ld * (N - 1) + D doubles
+    void in2d(const double* h, int32_t D, int64_t ld, int64_t N, const double** d) {
+        *d = map(h, Span::matrix(D, ld, N, 1, 0), true, false);
+    }
+    void out2d(double* h, int32_t D, int64_t ld, int64_t N, double** d, int64_t blocks = 1, int64_t block_stride = 0) {
+        *d = map(h, Span::matrix(D, ld, N, blocks, block_stride), false, true);
     }
     int finish() {
-        ahmc_ctx* ctx = ctx_;
-        for (auto& o : outs_) CU(cudaMemcpyAsync(o.h, o.d, o.bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        for (auto& o : outs_)
+            if (int rc = copy(o.h, o.d, o.span, o.elem, cudaMemcpyDeviceToHost)) return rc;
         return AHMC_OK;
     }
     bool host() const { return host_; }
 
 private:
-    struct Out { void* h; void* d; size_t bytes; };
-    template <class T>
-    T* map(T* h, size_t count, bool upload, bool download) {
-        if (!h || !host_) return h;
-        T* p = (T*)carver_.take<T>(count);
-        if (sizing_) return p;
-        if (upload && !rc_) rc_ = upload_now((void*)p, h, count * sizeof(T));
-        if (download) outs_.push_back({(void*)h, (void*)p, count * sizeof(T)});
-        return p;
-    }
-    int upload_now(void* d, const void* h, size_t bytes) {
+    // `blocks` blocks `block_stride` elements apart, each `rows` rows of `width` elements `pitch` apart
+    struct Span {
+        size_t width, pitch, rows, blocks, block_stride;
+        static Span flat(size_t count) { return {count, count, 1, 1, 0}; }
+        static Span matrix(int32_t D, int64_t ld, int64_t N, int64_t blocks, int64_t block_stride) {
+            if (N <= 0 || blocks <= 0) return flat(0);
+            if (ld != D) return {(size_t)D, (size_t)ld, (size_t)N, (size_t)blocks, (size_t)block_stride};
+            const size_t n = (size_t)D * N;  // no padding: each block is contiguous, and so are back-to-back blocks
+            return blocks == 1 || (size_t)block_stride == n ? flat(n * blocks) : Span{n, n, 1, (size_t)blocks, (size_t)block_stride};
+        }
+        size_t extent() const {
+            return blocks && rows ? block_stride * (blocks - 1) + pitch * (rows - 1) + width : 0;
+        }
+    };
+    struct Out { void* h; void* d; Span span; size_t elem; };
+    int copy(void* dst, const void* src, const Span& s, size_t elem, cudaMemcpyKind kind) {
         ahmc_ctx* ctx = ctx_;
-        CU(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, ctx->stream));
+        if (!s.extent()) return AHMC_OK;
+        for (size_t b = 0; b < s.blocks; ++b) {
+            const size_t off = b * s.block_stride * elem;
+            CU(copy_rows((char*)dst + off, (const char*)src + off, s.width * elem, s.pitch * elem, s.rows, kind, ctx->stream));
+        }
         return AHMC_OK;
+    }
+    template <class T>
+    T* map(T* h, const Span& s, bool upload, bool download) {
+        if (!h || !host_) return h;
+        T* p = (T*)carver_.take<T>(s.extent());
+        if (sizing_) return p;
+        if (upload && !rc_) rc_ = copy((void*)p, h, s, sizeof(T), cudaMemcpyHostToDevice);
+        if (download) outs_.push_back({(void*)h, (void*)p, s, sizeof(T)});
+        return p;
     }
     ahmc_ctx* ctx_;
     bool host_;
@@ -331,24 +366,25 @@ void stage_metric(Stager& st, const ahmc_metric* m, int32_t D, int64_t N, Metric
 
 // the phase-point fields the argument blocks share by name.  In: theta, r, -grad lp[, lp] of z (N chains).
 template <class Args>
-void stage_pp_in(Stager& st, const ahmc_phasepoint* z, int64_t N, Args& a, const double** lp_in = nullptr) {
-    const size_t c = (size_t)z->ld * N;
+void stage_pp_in(Stager& st, const ahmc_phasepoint* z, int32_t D, int64_t N, Args& a, const double** lp_in = nullptr) {
     a.ld_in = z->ld;
-    st.in((const double*)z->theta, c, &a.th_in);
-    st.in((const double*)z->r, c, &a.r_in);
-    st.in((const double*)z->lp_gradient, c, &a.g_in);
+    st.in2d((const double*)z->theta, D, z->ld, N, &a.th_in);
+    st.in2d((const double*)z->r, D, z->ld, N, &a.r_in);
+    st.in2d((const double*)z->lp_gradient, D, z->ld, N, &a.g_in);
     if (lp_in) st.in((const double*)z->lp_value, (size_t)N, lp_in);
 }
-// Out: `nv` doubles per vector field (ld * N, or a whole trajectory), `ns` per energy[, dH/dr from lk_gradient]
+// Out: every vector field D x N at z->ld, the energies N[, dH/dr from lk_gradient]; a trajectory has `steps` of each,
+// its vector fields `step_stride` doubles apart and its energies N apart
 template <class Args>
-void stage_pp_out(Stager& st, const ahmc_phasepoint* z, size_t nv, size_t ns, Args& a, double** dr_out = nullptr) {
+void stage_pp_out(Stager& st, const ahmc_phasepoint* z, int32_t D, int64_t N, Args& a, double** dr_out = nullptr,
+                  int64_t steps = 1, int64_t step_stride = 0) {
     a.ld_out = z->ld;
-    st.out(z->theta, nv, &a.th_out);
-    st.out(z->r, nv, &a.r_out);
-    st.out(z->lp_gradient, nv, &a.g_out);
-    if (dr_out) st.out(z->lk_gradient, nv, dr_out);
-    st.out(z->lp_value, ns, &a.lp_out);
-    st.out(z->lk_value, ns, &a.lk_out);
+    st.out2d(z->theta, D, z->ld, N, &a.th_out, steps, step_stride);
+    st.out2d(z->r, D, z->ld, N, &a.r_out, steps, step_stride);
+    st.out2d(z->lp_gradient, D, z->ld, N, &a.g_out, steps, step_stride);
+    if (dr_out) st.out2d(z->lk_gradient, D, z->ld, N, dr_out, steps, step_stride);
+    st.out(z->lp_value, (size_t)N * steps, &a.lp_out);
+    st.out(z->lk_value, (size_t)N * steps, &a.lk_out);
 }
 
 int finish_call(ahmc_ctx* ctx, Stager& st, uint32_t flags) {
@@ -926,14 +962,13 @@ int ahmc_phasepoint_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metri
     a.N = N;
     a.ld = z->ld;
     rc = st.stage([&](Stager& s) {
-        const size_t c = (size_t)z->ld * N;
         stage_metric(s, metric, D, N, &a.metric);
-        s.in((const double*)z->theta, c, &a.th);
-        s.in((const double*)z->r, c, &a.r);
+        s.in2d((const double*)z->theta, D, z->ld, N, &a.th);
+        s.in2d((const double*)z->r, D, z->ld, N, &a.r);
         s.out(z->lp_value, (size_t)N, &a.lp);
-        s.out(z->lp_gradient, c, &a.g);
+        s.out2d(z->lp_gradient, D, z->ld, N, &a.g);
         s.out(z->lk_value, (size_t)N, &a.lk);
-        s.out(z->lk_gradient, c, &a.dr);
+        s.out2d(z->lk_gradient, D, z->ld, N, &a.dr);
     });
     if (rc) return rc;
     int nl = 0;
@@ -1122,13 +1157,14 @@ static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const
     for (int64_t c0 = 0; c0 < N; c0 += chunk, ++k) {
         const int64_t n = (c0 + chunk <= N) ? chunk : N - c0;
         if (stage_in) {
-            CU(cudaMemcpyAsync(dTh + ldi * c0, z_in->theta + ldi * c0, (size_t)ldi * n * 8, cudaMemcpyHostToDevice, s_up));
+            CU(copy_rows(dTh + ldi * c0, z_in->theta + ldi * c0, (size_t)D * 8, (size_t)ldi * 8, (size_t)n, cudaMemcpyHostToDevice, s_up));
             if (eps_chain) CU(cudaMemcpyAsync(dEps + c0, eps_chain + c0, (size_t)n * 8, cudaMemcpyHostToDevice, s_up));
-            CU(cudaMemcpyAsync(dR + ldi * c0, z_in->r + ldi * c0, (size_t)ldi * n * 8, cudaMemcpyHostToDevice, s_up));
+            CU(copy_rows(dR + ldi * c0, z_in->r + ldi * c0, (size_t)D * 8, (size_t)ldi * 8, (size_t)n, cudaMemcpyHostToDevice, s_up));
             if (per_chain_minv)
                 CU(cudaMemcpyAsync(dMinv + metric->chain_stride * c0, metric->Minv + metric->chain_stride * c0,
                                    (size_t)metric->chain_stride * n * 8, cudaMemcpyHostToDevice, s_up));
-            if (has_g) CU(cudaMemcpyAsync(dG + ldi * c0, z_in->lp_gradient + ldi * c0, (size_t)ldi * n * 8, cudaMemcpyHostToDevice, s_up));
+            if (has_g)
+                CU(copy_rows(dG + ldi * c0, z_in->lp_gradient + ldi * c0, (size_t)D * 8, (size_t)ldi * 8, (size_t)n, cudaMemcpyHostToDevice, s_up));
             CU(cudaEventRecord(ctx->ev_in[k], s_up));
             CU(cudaStreamWaitEvent(s_cmp, ctx->ev_in[k], 0));
         }
@@ -1164,10 +1200,11 @@ static int leapfrog_host_pipelined(ahmc_ctx* ctx, const ahmc_model* model, const
         if (stage_out) {
             CU(cudaEventRecord(ctx->ev_k[k], s_cmp));
             CU(cudaStreamWaitEvent(s_down, ctx->ev_k[k], 0));
-            CU(cudaMemcpyAsync(z_out->theta + ldo * c0, a.th_out, (size_t)ldo * n * 8, cudaMemcpyDeviceToHost, s_down));
-            CU(cudaMemcpyAsync(z_out->r + ldo * c0, a.r_out, (size_t)ldo * n * 8, cudaMemcpyDeviceToHost, s_down));
-            CU(cudaMemcpyAsync(z_out->lp_gradient + ldo * c0, a.g_out, (size_t)ldo * n * 8, cudaMemcpyDeviceToHost, s_down));
-            if (a.dr_out) CU(cudaMemcpyAsync(z_out->lk_gradient + ldo * c0, a.dr_out, (size_t)ldo * n * 8, cudaMemcpyDeviceToHost, s_down));
+            const size_t w = (size_t)D * 8, pitch = (size_t)ldo * 8;  // rows d < D only: the caller's padding stays
+            CU(copy_rows(z_out->theta + ldo * c0, a.th_out, w, pitch, (size_t)n, cudaMemcpyDeviceToHost, s_down));
+            CU(copy_rows(z_out->r + ldo * c0, a.r_out, w, pitch, (size_t)n, cudaMemcpyDeviceToHost, s_down));
+            CU(copy_rows(z_out->lp_gradient + ldo * c0, a.g_out, w, pitch, (size_t)n, cudaMemcpyDeviceToHost, s_down));
+            if (a.dr_out) CU(copy_rows(z_out->lk_gradient + ldo * c0, a.dr_out, w, pitch, (size_t)n, cudaMemcpyDeviceToHost, s_down));
         }
     }
     ctx->launches += nl;
@@ -1256,8 +1293,8 @@ int ahmc_leapfrog_f64(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric*
     rc = st.stage([&](Stager& s) {
         stage_metric(s, metric, D, N, &a.metric);
         s.in(eps_chain, (size_t)N, &a.eps_chain);
-        stage_pp_in(s, z_in, N, a);
-        stage_pp_out(s, z_out, (size_t)z_out->ld * N, (size_t)N, a, &a.dr_out);
+        stage_pp_in(s, z_in, D, N, a);
+        stage_pp_out(s, z_out, D, N, a, &a.dr_out);
         s.out(status, (size_t)N, &a.status);
         s.out(steps_done, (size_t)N, &a.steps_done);
     });
@@ -1326,7 +1363,7 @@ int ahmc_rand_momentum_f64(ahmc_ctx* ctx, const ahmc_metric* metric, int32_t D, 
     rc = st.stage([&](Stager& s) {
         stage_metric(s, metric, D, N, &a.metric);
         s.in(rng->normal_tape, (size_t)D * N, &a.normal_tape);
-        s.out(r, (size_t)ld * N, &a.r);
+        s.out2d(r, D, ld, N, &a.r);
     });
     if (rc) return rc;
     int nl = 0;
@@ -1336,7 +1373,10 @@ int ahmc_rand_momentum_f64(ahmc_ctx* ctx, const ahmc_metric* metric, int32_t D, 
 }
 
 // ---------------------------------------------------------------------------------------------- transitions
-static void stage_stats(Stager& st, const ahmc_stats* s, int64_t N, StatsDev* d) {
+// the statistics a sampler writes: max_hamiltonian_energy_error NUTS only (`max_dH`), tree_depth NUTS and the multinomial
+// draw's offset (`depth`).  A field it does not write is not staged, so a host-buffer call leaves the caller's array as
+// it was, as a device-pointer call does
+static void stage_stats(Stager& st, const ahmc_stats* s, int64_t N, StatsDev* d, bool max_dH, bool depth) {
     memset(d, 0, sizeof *d);
     if (!s) return;
     st.out(s->n_steps, (size_t)N, &d->n_steps);
@@ -1345,8 +1385,8 @@ static void stage_stats(Stager& st, const ahmc_stats* s, int64_t N, StatsDev* d)
     st.out(s->log_density, (size_t)N, &d->log_density);
     st.out(s->hamiltonian_energy, (size_t)N, &d->hamiltonian_energy);
     st.out(s->hamiltonian_energy_error, (size_t)N, &d->hamiltonian_energy_error);
-    st.out(s->max_hamiltonian_energy_error, (size_t)N, &d->max_hamiltonian_energy_error);
-    st.out(s->tree_depth, (size_t)N, &d->tree_depth);
+    if (max_dH) st.out(s->max_hamiltonian_energy_error, (size_t)N, &d->max_hamiltonian_energy_error);
+    if (depth) st.out(s->tree_depth, (size_t)N, &d->tree_depth);
     st.out(s->numerical_error, (size_t)N, &d->numerical_error);
 }
 
@@ -1532,10 +1572,10 @@ static int hmc_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* m
         stage_metric(s, metric, D, N, &a.metric);
         if (cfg) stage_adapt(s, metric, cfg, D, N, n_transitions, &h.ad, &a.eps_chain);
         else s.in(eps_chain, (size_t)N, &a.eps_chain);
-        stage_pp_in(s, z_in, N, a, &a.lp_in);
-        stage_pp_out(s, z_out, (size_t)z_out->ld * N, (size_t)N, a);
+        stage_pp_in(s, z_in, D, N, a, &a.lp_in);
+        stage_pp_out(s, z_out, D, N, a);
         stage_rng(s, rng, D, N, false, &h.rng);
-        stage_stats(s, stats, N * n_transitions, &h.st);
+        stage_stats(s, stats, N * n_transitions, &h.st, false, false);
         s.out(draws, (size_t)D * N * n_transitions, &h.draws);
     });
     if (rc) return rc;
@@ -1616,10 +1656,10 @@ static int nuts_impl(ahmc_ctx* ctx, const ahmc_model* model, const ahmc_metric* 
         stage_metric(s, metric, D, N, &a.metric);
         if (cfg) stage_adapt(s, metric, cfg, D, N, n_transitions, &a.ad, &a.eps_chain);
         else s.in(eps_chain, (size_t)N, &a.eps_chain);
-        stage_pp_in(s, z_in, N, a, &a.lp_in);
-        stage_pp_out(s, z_out, (size_t)z_out->ld * N, (size_t)N, a);
+        stage_pp_in(s, z_in, D, N, a, &a.lp_in);
+        stage_pp_out(s, z_out, D, N, a);
         stage_rng(s, rng, D, N, true, &a.rng);
-        stage_stats(s, stats, N * n_transitions, &a.st);
+        stage_stats(s, stats, N * n_transitions, &a.st, true, true);
         s.out(draws, (size_t)D * N * n_transitions, &a.draws);
     });
     if (rc) return rc;
@@ -1673,8 +1713,8 @@ int ahmc_leapfrog_trajectory_f64(ahmc_ctx* ctx, const ahmc_model* model, const a
     rc = st.stage([&](Stager& s) {
         stage_metric(s, metric, D, N, &a.metric);
         s.in(eps_chain, (size_t)N, &a.eps_chain);
-        stage_pp_in(s, z_in, N, a);
-        stage_pp_out(s, traj, (size_t)step_stride * n_abs, (size_t)N * n_abs, a, &a.dr_out);
+        stage_pp_in(s, z_in, D, N, a);
+        stage_pp_out(s, traj, D, N, a, &a.dr_out, n_abs, step_stride);
         s.out(steps_done, (size_t)N, &a.steps_done);
     });
     if (rc) return rc;
@@ -1712,10 +1752,10 @@ int ahmc_hmc_multinomial_transition_f64(ahmc_ctx* ctx, const ahmc_model* model, 
     rc = st.stage([&](Stager& s) {
         stage_metric(s, metric, D, N, &a.metric);
         s.in(eps_chain, (size_t)N, &a.eps_chain);
-        stage_pp_in(s, z_in, N, a, &a.lp_in);
-        stage_pp_out(s, z_out, (size_t)z_out->ld * N, (size_t)N, a);
+        stage_pp_in(s, z_in, D, N, a, &a.lp_in);
+        stage_pp_out(s, z_out, D, N, a);
         stage_rng(s, rng, D, N, false, &a.rng);
-        stage_stats(s, stats, N, &a.st);
+        stage_stats(s, stats, N, &a.st, false, true);
     });
     if (rc) return rc;
     if ((rc = ensure(ctx, ctx->energy_ws, (size_t)(n_steps + 1) * (size_t)N * sizeof(double), "the multinomial energy tape")))
@@ -1789,7 +1829,7 @@ int ahmc_adapt_summary_f64(ahmc_ctx* ctx, int32_t D, int64_t N, const double* th
     const double *d_theta, *d_alpha;
     double* d_out;
     rc = st.stage([&](Stager& s) {
-        s.in(theta, (size_t)ld * N, &d_theta);
+        s.in2d(theta, D, ld, N, &d_theta);
         s.in(acceptance_rate, (size_t)N, &d_alpha);
         s.out(out, (size_t)(2 + 2 * D), &d_out);
     });
@@ -1809,7 +1849,7 @@ int ahmc_adapt_cov_f64(ahmc_ctx* ctx, int32_t D, int64_t N, const double* theta,
     const double *d_theta, *d_mean;
     double* d_out;
     int rc = st.stage([&](Stager& s) {
-        s.in(theta, (size_t)ld * N, &d_theta);
+        s.in2d(theta, D, ld, N, &d_theta);
         s.in(mean, (size_t)D, &d_mean);
         s.out(out, (size_t)D * D, &d_out);
     });
@@ -1847,14 +1887,13 @@ int ahmc_find_good_stepsize_f64(ahmc_ctx* ctx, const ahmc_model* model, const ah
     a.eps0 = initial_step_size;
     a.max_iters = max_n_iters;
     rc = st.stage([&](Stager& s) {
-        const size_t c = (size_t)z->ld * N;
         stage_metric(s, metric, D, N, &a.metric);
-        s.in((const double*)z->theta, c, &a.th);
-        s.in((const double*)z->lp_gradient, c, &a.g);
+        s.in2d((const double*)z->theta, D, z->ld, N, &a.th);
+        s.in2d((const double*)z->lp_gradient, D, z->ld, N, &a.g);
         s.in((const double*)z->lp_value, (size_t)N, &a.lp);
         s.in(rng->normal_tape, (size_t)D * N, &a.normal_tape);
         s.out(eps_out, (size_t)N, &a.eps_out);
-        s.out(r_out, c, &a.r_out);
+        s.out2d(r_out, D, z->ld, N, &a.r_out);
     });
     if (rc) return rc;
     if (D > 512 && (rc = chain_workspace(ctx, (size_t)kBigFindEpsVectors * D * (size_t)N * sizeof(double), &a.scratch))) return rc;

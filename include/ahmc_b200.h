@@ -9,7 +9,9 @@
  *    DATA, never an error: non-finite energies are mapped to -Inf exactly like the PhasePoint
  *    constructor (src/hamiltonian.jl:95-104) and reported in per-chain status/statistics.
  *  - Arrays are Julia column-major D x N: element (d, chain c) at `d + ld*c` (each chain contiguous).
- *    Unless AHMC_FLAG_HOST_BUFFERS is passed every array pointer is a DEVICE pointer (e.g. the
+ *    The library reads and writes rows d < D only: the padding rows D..ld-1 of every chain are never
+ *    touched (a `view(X, 1:D, :)` of a taller matrix works), and a D x N argument needs ld*(N-1) + D
+ *    doubles.  Unless AHMC_FLAG_HOST_BUFFERS is passed every array pointer is a DEVICE pointer (e.g. the
  *    `pointer(::CuArray)` of the reference's CUDA extension, ext/AdvancedHMCCUDAExt.jl).
  *    With AHMC_FLAG_HOST_BUFFERS they are host pointers; the library stages them through pinned
  *    memory on the context stream (host->device, kernels, device->host inside the call).

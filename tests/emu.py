@@ -27,6 +27,10 @@ def P(a):
 
 
 # ------------------------------------------------------------------------------------------------ request structs
+# the last fields of the trajectory harnesses' requests: leading dimensions of the D x N inputs and outputs (0: D)
+_LD = [("ld_in", C.c_int64), ("ld_out", C.c_int64)]
+
+
 class EmuNuts(C.Structure):
     _fields_ = [("model_kind", C.c_int32), ("metric_kind", C.c_int32), ("D", C.c_int32), ("N", C.c_int64), ("p0", _vp), ("p1", _vp),
                 ("c0", C.c_double), ("Minv", _vp), ("minv_stride", C.c_int64), ("cholU", _vp), ("eps", C.c_double),
@@ -39,7 +43,7 @@ class EmuNuts(C.Structure):
                 ("adapt", C.c_int32), ("n_adapts", C.c_int32), ("init_buffer", C.c_int32), ("term_buffer", C.c_int32),
                 ("window_size", C.c_int32), ("delta", C.c_double), ("gamma", C.c_double), ("t0", C.c_double), ("kappa", C.c_double),
                 ("adapt_metric", C.c_int32), ("n_min", C.c_int32), ("eps_rw", _vp), ("minv_rw", _vp), ("eps_trace", _vp),
-                ("temper_alpha", C.c_double), ("coop_padded", C.c_int32)]
+                ("temper_alpha", C.c_double), ("coop_padded", C.c_int32), *_LD]
 
 
 class EmuLf(C.Structure):
@@ -49,14 +53,14 @@ class EmuLf(C.Structure):
                 ("r_in", _vp), ("g_in", _vp), ("lp_in", _vp), ("th_out", _vp), ("r_out", _vp), ("g_out", _vp), ("lp_out", _vp),
                 ("lk_out", _vp), ("dr_out", _vp), ("status", _vp), ("steps_done", _vp), ("flags", C.c_uint32), ("hmc", C.c_int32),
                 ("refresh", C.c_int32), ("n_transitions", C.c_int32), ("seed", C.c_uint64), ("offset", C.c_uint64),
-                ("normal_tape", _vp), ("exp_tape", _vp), ("is_accept", _vp), ("acc", _vp), ("dH", _vp), ("draws", _vp)]
+                ("normal_tape", _vp), ("exp_tape", _vp), ("is_accept", _vp), ("acc", _vp), ("dH", _vp), ("draws", _vp), *_LD]
 
 
 class EmuMn(C.Structure):
     _fields_ = [("model_kind", C.c_int32), ("metric_kind", C.c_int32), ("D", C.c_int32), ("N", C.c_int64), ("p0", _vp), ("p1", _vp),
                 ("Minv", _vp), ("cholU", _vp), ("eps", C.c_double), ("n_steps", C.c_int32), ("n_fwd", C.c_int32),
                 ("normal_tape", _vp), ("unif_tape", _vp), ("th_in", _vp), ("g_in", _vp), ("lp_in", _vp), ("th_out", _vp),
-                ("r_out", _vp), ("g_out", _vp), ("lp_out", _vp), ("lk_out", _vp), ("acc", _vp), ("index", _vp), ("temper_alpha", C.c_double)]
+                ("r_out", _vp), ("g_out", _vp), ("lp_out", _vp), ("lk_out", _vp), ("acc", _vp), ("index", _vp), ("temper_alpha", C.c_double), *_LD]
 
 
 class EmuDense(C.Structure):
@@ -64,7 +68,7 @@ class EmuDense(C.Structure):
                 ("Mdiag", _vp), ("eps", C.c_double), ("eps_chain", _vp), ("n_steps", C.c_int32), ("fwd", C.c_int32),
                 ("th_in", _vp), ("r_in", _vp), ("g_in", _vp), ("th_out", _vp), ("r_out", _vp), ("g_out", _vp), ("dr_out", _vp),
                 ("lp_out", _vp), ("lk_out", _vp), ("status", _vp), ("steps_done", _vp), ("need_exact", _vp),
-                ("wide_tile", C.c_int32), ("norms_out", C.c_double * 2)]
+                ("wide_tile", C.c_int32), ("norms_out", C.c_double * 2), *_LD]
 
 
 class EmuGlm(C.Structure):
@@ -72,7 +76,7 @@ class EmuGlm(C.Structure):
                 ("c0", C.c_double), ("Minv", _vp), ("chain_stride", C.c_int64), ("eps", C.c_double), ("eps_chain", _vp),
                 ("n_steps", C.c_int32), ("fwd", C.c_int32), ("th_in", _vp), ("r_in", _vp), ("g_in", _vp), ("th_out", _vp),
                 ("r_out", _vp), ("g_out", _vp), ("dr_out", _vp), ("lp_out", _vp), ("lk_out", _vp), ("status", _vp),
-                ("steps_done", _vp), ("nc_out", C.c_int32), ("stages_out", C.c_int32)]
+                ("steps_done", _vp), ("nc_out", C.c_int32), ("stages_out", C.c_int32), *_LD]
 
 
 class EmuBigd(C.Structure):

@@ -54,6 +54,7 @@ struct EmuDense {
     uint8_t* need_exact;
     int32_t wide_tile;  // RB == 2 only: 1 -> the <2,4> (32-chain) form instead of the default <2,2,2>
     double norms_out[2];
+    int64_t ld_in, ld_out;  // leading dimensions of the D x N inputs / outputs (0: D)
 };
 EMU_EXPORT_SIZEOF(EmuDense);
 
@@ -86,9 +87,9 @@ extern "C" int emu_dense(EmuDense* q) {
     DenseArgs a{};
     a.D = q->D; a.Dp = Dp; a.N = q->N; a.P = q->P ? Pp.data() : nullptr; a.w = q->w; a.mu = q->mu; a.c0 = q->c0;
     a.Minv = q->Minv ? Mp.data() : nullptr; a.Mdiag = q->Mdiag; a.norms = norms; a.eps = q->eps; a.eps_chain = q->eps_chain;
-    a.n_steps = q->n_steps; a.fwd = q->fwd; a.th_in = q->th_in; a.r_in = q->r_in; a.g_in = q->g_in; a.ld_in = q->D;
+    a.n_steps = q->n_steps; a.fwd = q->fwd; a.th_in = q->th_in; a.r_in = q->r_in; a.g_in = q->g_in; a.ld_in = q->ld_in ? q->ld_in : q->D;
     a.th_out = q->th_out; a.r_out = q->r_out; a.g_out = q->g_out; a.dr_out = q->dr_out; a.lp_out = q->lp_out; a.lk_out = q->lk_out;
-    a.ld_out = q->D; a.status = q->status; a.steps_done = q->steps_done; a.need_exact = q->need_exact;
+    a.ld_out = q->ld_out ? q->ld_out : q->D; a.status = q->status; a.steps_done = q->steps_done; a.need_exact = q->need_exact;
     void (*fn)(const void*) = nullptr;
     int CB = 0;  // the instantiation's, as launch_dense_traj picks it (RB == 2 may ask for the 32-chain form instead)
     if (RB == 1) fn = dense_thunk<1, 4, 1>, CB = 4;

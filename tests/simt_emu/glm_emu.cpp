@@ -36,6 +36,7 @@ struct EmuGlm {
     uint32_t* status;
     int32_t* steps_done;
     int32_t nc_out, stages_out;
+    int64_t ld_in, ld_out;  // leading dimensions of the D x N inputs / outputs (0: D)
 };
 EMU_EXPORT_SIZEOF(EmuGlm);
 
@@ -51,9 +52,9 @@ extern "C" int emu_glm(EmuGlm* e) {
     for (int i = 0; i < e->n; ++i) std::memcpy(Xp.data() + (size_t)i * lds, e->X + (size_t)i * e->D, sizeof(double) * e->D);
     a.family = e->family; a.D = e->D; a.n = e->n; a.N = e->N; a.Xp = Xp.data(); a.y = e->y; a.prec = e->prec; a.c0 = e->c0;
     a.Minv = e->Minv; a.chain_stride = e->chain_stride; a.eps = e->eps; a.eps_chain = e->eps_chain;
-    a.n_steps = e->n_steps; a.fwd = e->fwd; a.th_in = e->th_in; a.r_in = e->r_in; a.g_in = e->g_in; a.ld_in = e->D;
+    a.n_steps = e->n_steps; a.fwd = e->fwd; a.th_in = e->th_in; a.r_in = e->r_in; a.g_in = e->g_in; a.ld_in = e->ld_in ? e->ld_in : e->D;
     a.th_out = e->th_out; a.r_out = e->r_out; a.g_out = e->g_out; a.dr_out = e->dr_out; a.lp_out = e->lp_out; a.lk_out = e->lk_out;
-    a.ld_out = e->D; a.status = e->status; a.steps_done = e->steps_done;
+    a.ld_out = e->ld_out ? e->ld_out : e->D; a.status = e->status; a.steps_done = e->steps_done;
     void (*fn)(const void*) = nullptr;
     const bool logit = e->family == AHMC_GLM_BERNOULLI_LOGIT;
     if (CB != 2) return -2;

@@ -27,6 +27,7 @@ struct EmuMn {
     double* acc;
     int32_t* index;
     double temper_alpha;
+    int64_t ld_in, ld_out;  // leading dimensions of the D x N inputs / outputs (0: D)
 };
 EMU_EXPORT_SIZEOF(EmuMn);
 
@@ -48,7 +49,8 @@ extern "C" int emu_multinomial(const EmuMn* q) {
     else if (D <= 8) G = 8, E = 1;
     else if (D > 32 && D <= 64) G = 32, E = 2;
     else return -1;
-    std::vector<double> r_in((size_t)D * q->N, 0.0), energies((size_t)(q->n_steps + 1) * q->N, 0.0);
+    const int64_t ld_in = q->ld_in ? q->ld_in : D;
+    std::vector<double> r_in((size_t)ld_in * q->N, 0.0), energies((size_t)(q->n_steps + 1) * q->N, 0.0);
     MultinomialArgs a{};
     a.model = ModelDev{q->model_kind, D, q->p0, q->p1, 0.0};
     a.metric = MetricDev{q->metric_kind, q->Minv, 0, q->cholU};
@@ -60,9 +62,9 @@ extern "C" int emu_multinomial(const EmuMn* q) {
     a.refresh = 1;
     a.rng = RngDev{1, 0, q->normal_tape, q->unif_tape, 1, nullptr, 0, 0.0, q->temper_alpha};
     a.th_in = q->th_in; a.r_in = r_in.data(); a.g_in = q->g_in; a.lp_in = q->lp_in;
-    a.ld_in = D;
+    a.ld_in = ld_in;
     a.th_out = q->th_out; a.r_out = q->r_out; a.g_out = q->g_out; a.lp_out = q->lp_out; a.lk_out = q->lk_out;
-    a.ld_out = D;
+    a.ld_out = q->ld_out ? q->ld_out : D;
     a.st = StatsDev{};
     a.st.acceptance_rate = q->acc;
     a.st.tree_depth = q->index;

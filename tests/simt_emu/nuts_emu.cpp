@@ -47,6 +47,7 @@ struct EmuNuts {
     double *eps_rw, *minv_rw, *eps_trace;
     double temper_alpha;
     int32_t coop_padded;  // 1: also hand the kernel column-padded copies of the dense matrices (one bulk copy per chunk)
+    int64_t ld_in, ld_out;  // leading dimensions of the D x N inputs / outputs (0: D)
 };
 EMU_EXPORT_SIZEOF(EmuNuts);
 
@@ -157,9 +158,9 @@ extern "C" int emu_nuts(const EmuNuts* q) {
     a.rng = RngDev{q->seed, q->offset, q->normal_tape, q->exp_tape, q->exp_stride, q->dir_tape, q->dir_stride, q->partial_alpha, q->temper_alpha};
     a.refresh = q->refresh;
     a.th_in = q->th_in; a.r_in = q->r_in; a.g_in = q->g_in; a.lp_in = q->lp_in;
-    a.ld_in = D;
+    a.ld_in = q->ld_in ? q->ld_in : D;
     a.th_out = q->th_out; a.r_out = q->r_out; a.g_out = q->g_out; a.lp_out = q->lp_out; a.lk_out = q->lk_out;
-    a.ld_out = D;
+    a.ld_out = q->ld_out ? q->ld_out : D;
     a.st = StatsDev{};
     a.st.n_steps = q->n_steps;
     a.st.tree_depth = q->tree_depth;

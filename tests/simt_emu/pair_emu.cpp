@@ -24,9 +24,9 @@ extern "C" int emu_leapfrog_pair(const EmuLf* q) {
     a.n_steps = q->n_steps;
     a.fwd = q->fwd;
     a.th_in = q->th_in; a.r_in = q->r_in; a.g_in = q->g_in; a.lp_in = q->lp_in;
-    a.ld_in = D;
+    a.ld_in = q->ld_in ? q->ld_in : D;
     a.th_out = q->th_out; a.r_out = q->r_out; a.g_out = q->g_out; a.lp_out = q->lp_out; a.lk_out = q->lk_out; a.dr_out = q->dr_out;
-    a.ld_out = D;
+    a.ld_out = q->ld_out ? q->ld_out : D;
     a.status = q->status;
     a.steps_done = q->steps_done;
     a.flags = q->flags;
